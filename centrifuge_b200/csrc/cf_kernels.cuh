@@ -3,7 +3,7 @@
 // Work decomposition (one batch of units = reads or pairs), DESIGN.md section 4:
 //   k_pack       reads (1 byte/base) -> 2-bit strands in search order + N masks
 //   k_search_t   FM-index backward search, the hot loop: ONE THREAD per (unit, mate, strand) greedy walk over the
-//                re-cut device index (rank16: one 16-byte gather per rank query; K-mer, death-depth and walk8 tables
+//                re-cut device index (rank16: one 16-byte gather per rank query; K-mer (with its death bitmap) and walk8 tables
 //                delete dependent gathers); one fetch point per loop iteration for all 32 walks of a warp
 //   k_search<G>  the warp-cooperative A/B variant (G lanes per walk on the file's 128-byte sides, shuffle popcount):
 //                same results, issue-bound and several times slower; uses the

@@ -25,7 +25,7 @@
 namespace cfb {
 
 static const uint64_t kOff = 0xffffffffffffffffull;
-static const uint64_t kUnk = 0xfffffffffffffffeull;   // HitRec.top == bot == kUnk: a hit shorter than min_hitlen whose SA range was not computed (death-depth table)
+static const uint64_t kUnk = 0xfffffffffffffffeull;   // HitRec.top == bot == kUnk: a hit shorter than min_hitlen whose SA range was not computed (death bitmap of the K-mer table)
 static const uint32_t kBwNone = 0xffffffffu;       // BWTHit::reset(): _bwoff = OFF_MASK
 
 // ----------------------------------------------------------------------------------------
@@ -52,11 +52,10 @@ struct IndexView {
 	const uint64_t* ftab2;          // device-only fused ftab: (top, bot) per 10-mer, eftab already resolved
 	const uint16_t* rtab16;         // device-only resolve table: sequence id of EVERY SA row (one of rtab16/rtab32, or neither)
 	const uint32_t* rtab32;
-	const uint64_t* ftabk;          // device-only extended jump table: (top, bot) per K-mer, K = ftabk_chars (0 = absent)
+	const uint64_t* ftabk;          // device-only K-mer jump table: (top | width << 40, death bitmap) per K-mer, K = ftabk_chars, see k_build_ftabk (null = absent)
 	const uint64_t* walk8;          // device-only: per SA row, the row 8 LF steps on | the 8 BWT bases met << 40 | #valid steps << 56 (null = absent)
 	uint64_t walk8_rows;            // rows [0, walk8_rows) have a walk8 entry (the table may cover a prefix of the rows when HBM is short)
-	const uint8_t*  ftabd;          // device-only "death depth" table: 2 bits per (D = base K + 3)-mer, see k_build_ftabd (null = absent)
-	int32_t  ftabd_chars, ftabd_base;   // D and the K of the jump table it extends (ftabk_chars, or ftab_chars without a K-mer table)
+	int32_t  ftabd_chars;           // K + 3 while the K-mer table carries the death bitmap, else 0
 	uint64_t len, zoff, zside, fchr[4], last_boundary, num_sides, num_blocks;
 	uint32_t zoffc, n_boundaries, n_seqs, n_host;
 	int32_t  off_rate, ftab_chars, bshift, ftabk_chars;
@@ -81,7 +80,8 @@ static const uint64_t kRowMask = (1ull << 40) - 1ull, kRowStart = 1ull << 63, kR
 struct Counters {   // algorithmic-operation counters (SURVEY.md section 8d definition)
 	unsigned long long units, partial_searches, ftab_probes, sides_search, walk_steps, rows_resolved, lf_steps, ext_searches;
 	// the product's own load requests (count mode 2: every derived table live, one entry per lane-level gather):
-	// rank16 entries (16 B), 10-mer table entries (16 B), K-mer table entries (16 B), walk8 entries (8 B)
+	// rank16 entries (16 B), 10-mer table entries (16 B), K-mer table entries (16 B), walk8 entries (8 B); req_ftabd stays 0
+	// (the death bitmap is read with the K-mer table entry)
 	unsigned long long req_rank16, req_ftab2, req_ftabk, req_walk8, req_ftabd;
 };
 

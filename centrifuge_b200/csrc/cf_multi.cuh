@@ -247,7 +247,8 @@ __global__ void __launch_bounds__(128) k_gather_probe_bulk(const ulonglong2* __r
 	}
 	if(acc == 0x123456789abcull) *sink = acc;
 }
-// table: 0 = rank16 (16-byte entries), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it)
+// table: 0 = rank16 (16-byte entries), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it),
+// 4 = death bits, which have no table of their own (always "not built")
 extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_requests, double* g_requests_per_s, double* ms_out) {
 	if(!ix || !g_requests_per_s || ix->device < 0) return fail(CFB_EINVAL, "cfb_gather_ceiling: bad argument");
 	CK(cudaSetDevice(ix->device));
@@ -258,7 +259,7 @@ extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_req
 		case 1: base = (const unsigned long long*)v.ftabk; n = t.ftabk_bytes / 16; W = 2; break;
 		case 2: base = (const unsigned long long*)v.walk8; n = t.walk8_bytes / 8; W = 1; break;
 		case 3: base = v.rtab32 ? (const unsigned long long*)v.rtab32 : (const unsigned long long*)v.rtab16; n = t.resolve_table_bytes / 8; W = 1; break;
-		case 4: base = (const unsigned long long*)v.ftabd; n = t.ftabd_bytes / 8; W = 1; break;
+		case 4: break;      // death bits: no table of their own, they live in the K-mer table's entries
 		default: return fail(CFB_EINVAL, "cfb_gather_ceiling: unknown table %d", table);
 	}
 	if(!base || n == 0) return fail(CFB_EINVAL, "cfb_gather_ceiling: table %d is not built", table);

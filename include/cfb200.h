@@ -67,17 +67,17 @@ int cfb_index_get_info(const cfb_index*, cfb_index_info* out);
 
 /* What the device replica holds (bytes of HBM each; 0 = not built).  The derived tables are built at load time in
  * this order of benefit per byte, each only while it fits the budget left after the batch head-room (12 GB unless
- * CFB_HBM_HEADROOM_GB says otherwise; DESIGN.md 3): rank16 + ftab2 (always), the K-mer jump table, the resolve
- * table, the death-depth table, walk8 (possibly for a prefix of the rows).  The file's sides are dropped once rank16 exists (sides_bytes = 0)
+ * CFB_HBM_HEADROOM_GB says otherwise; DESIGN.md 3): rank16 + ftab2 (always), the K-mer jump table (whose 16-byte entries
+ * also carry the death bitmap), the resolve table, walk8 (possibly for a prefix of the rows).  The file's sides are dropped once rank16 exists (sides_bytes = 0)
  * except on small indexes, where the sides-based A/B kernels and test hooks stay usable. */
 typedef struct {
 	uint64_t sides_bytes, sample_bytes, rank16_bytes, ftab2_bytes, ftabk_bytes, resolve_table_bytes, walk8_bytes;
 	uint64_t total_bytes, free_bytes_after_load;
 	uint64_t walk8_rows;            /* rows [0, walk8_rows) have a walk8 entry (all rows when HBM allows, else a prefix) */
-	uint64_t ftabd_bytes;           /* death-depth table: 2 bits per (K+3)-mer = 16 bytes per K-mer */
-	int32_t  ftabk_chars;           /* K of the jump table, 0 = none */
+	uint64_t ftabd_bytes;           /* always 0: the death bitmap (1 bit per (K+3)-mer) lives in the K-mer table's entries */
+	int32_t  ftabk_chars;           /* K of the jump table, 0 = none (= ftab_chars when it is built for the death bitmap alone) */
 	int32_t  resolve_entry_bytes;   /* 2 or 4, 0 = no resolve table (rows are resolved by walking) */
-	int32_t  ftabd_chars;           /* K + 3 of the death-depth table, 0 = none */
+	int32_t  ftabd_chars;           /* K + 3 while the K-mer table carries the death bitmap, 0 = none */
 	int32_t  pad;
 } cfb_index_tables;
 int cfb_index_get_tables(const cfb_index*, cfb_index_tables* out);
@@ -249,9 +249,9 @@ int cfb_comm_info(const cfb_ctx*, int* rank, int* size, int* nccl_version);
 int cfb_counts_allreduce(cfb_ctx* const* ctxs, int n, uint64_t* dense_out, uint64_t cap);
 
 /* Measurement hooks (bench.py): the product's own load requests of the last batch when the context was created with
- * CFB_COUNT=2 -- {rank16 entries, 10-mer table entries, K-mer table entries, walk8 entries, death-depth bytes} -- and the random-gather
+ * CFB_COUNT=2 -- {rank16 entries, 10-mer table entries, K-mer table entries, walk8 entries, 0} -- and the random-gather
  * ceiling of this device over the replica's own arrays: independent uniformly random gathers from table 0 = rank16
- * (16 B), 1 = K-mer table (16 B), 2 = walk8 (8 B), 3 = resolve table (8 B), 4 = death-depth table (8 B), in G requests/s. */
+ * (16 B), 1 = K-mer table (16 B), 2 = walk8 (8 B), 3 = resolve table (8 B), in G requests/s; 4 (death bits: no table of their own) always fails as not built. */
 int cfb_ctx_requests(cfb_ctx*, uint64_t out[5]);
 int cfb_gather_ceiling(const cfb_index*, int table, uint64_t n_requests, double* g_requests_per_s, double* ms);
 

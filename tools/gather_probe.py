@@ -15,10 +15,9 @@ base, d = bench.get_index(a)
 ix = capi.Index(base, 0)
 tb = ix.tables()
 print("index replica: %.1f GB in HBM; tables %s" % (tb["total_bytes"] / 1e9, {k: v for k, v in tb.items() if k.endswith("chars") or k == "walk8_rows"}))
-names = {0: "rank16 (16 B entries, %.1f GB)" % (tb["rank16_bytes"] / 1e9), 1: "K-mer table (16 B entries, %.1f GB)" % (tb["ftabk_bytes"] / 1e9),
-         2: "walk8 (8 B entries, %.1f GB)" % (tb["walk8_bytes"] / 1e9), 3: "resolve table (8 B words, %.1f GB)" % (tb["resolve_table_bytes"] / 1e9),
-         4: "death-depth table (8 B words, %.1f GB)" % (tb["ftabd_bytes"] / 1e9)}
-for t in (0, 1, 2, 3, 4):
+names = {0: "rank16 (16 B entries, %.1f GB)" % (tb["rank16_bytes"] / 1e9), 1: "K-mer table + death bitmap (16 B entries, %.1f GB)" % (tb["ftabk_bytes"] / 1e9),
+         2: "walk8 (8 B entries, %.1f GB)" % (tb["walk8_bytes"] / 1e9), 3: "resolve table (8 B words, %.1f GB)" % (tb["resolve_table_bytes"] / 1e9)}
+for t in (0, 1, 2, 3):
     try:
         g, ms = capi.gather_ceiling(ix, t, 1 << 31)
         print("LDG   %-45s %7.2f G requests/s  (%.1f ms)" % (names[t], g, ms))
