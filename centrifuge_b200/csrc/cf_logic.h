@@ -470,8 +470,12 @@ struct EmitRows {       // second pass: write the SA rows to resolve, in consump
 	}
 };
 
+// Sequence ids are 32-bit, so uniqueID is too; the reference's OFF (a node merged by the tree reduction) is kUidOff, which is
+// never below n_seqs.  64 bytes instead of 72 lets k_score keep more hit maps in shared memory.
+static const uint32_t kUidOff = 0xffffffffu;
 struct Entry {          // HitCount classifier.h:31-57 (fields that influence output)
-	uint64_t uniqueID, taxID;
+	uint64_t taxID;
+	uint32_t uniqueID;
 	uint32_t scores[2][2], lens[2][2];
 	uint32_t score, hitlen, ts;
 	int32_t  pid;        // path id or -1 (empty path)
@@ -518,7 +522,7 @@ CFB_HDN uint32_t score_plan(const IndexView& v, const Params& p, const uint64_t*
 			}
 			uint32_t idx = 0;
 			for(; idx < nmap; ++idx) {
-				const bool same = rank == 0 ? ((uint64_t)ref == map[idx].uniqueID) : (taxID == map[idx].taxID);
+				const bool same = rank == 0 ? (ref == map[idx].uniqueID) : (taxID == map[idx].taxID);
 				if(same) {
 					if(map[idx].ts != ts) { map[idx].scores[rdi][fwi] += sc; map[idx].lens[rdi][fwi] += (uint32_t)hl; map[idx].ts = ts; }
 					break;
@@ -594,7 +598,7 @@ CFB_HDN uint32_t reduce_and_emit(const IndexView& v, const Params& p, bool paire
 					Entry& h = map[i];
 					if(h.rank != rank) continue;
 					const uint64_t cur_parent = ((uint32_t)rank + 1 >= path_size(h)) ? 1 : path_at(v, h, rank + 1);
-					if(parent == cur_parent) { h.uniqueID = kOff; h.rank = rank + 1; h.taxID = parent; }
+					if(parent == cur_parent) { h.uniqueID = kUidOff; h.rank = rank + 1; h.taxID = parent; }
 				}
 				bool first = true;
 				for(uint32_t i = 0; i < nmap; i++) {
@@ -614,7 +618,7 @@ CFB_HDN uint32_t reduce_and_emit(const IndexView& v, const Params& p, bool paire
 	for(uint32_t i = 0; i < nmap; i++) {
 		if(only_host && !is_host(v, map[i].taxID)) continue;
 		OutRec r; r.taxid = map[i].taxID; r.score = map[i].score; r.hitlen = map[i].hitlen;
-		r.uid = map[i].uniqueID < (uint64_t)v.n_seqs ? (uint32_t)map[i].uniqueID : 0xFFFFFFFFu; r.pad = 0;
+		r.uid = map[i].uniqueID < v.n_seqs ? map[i].uniqueID : 0xFFFFFFFFu; r.pad = 0;
 		out[no++] = r;
 	}
 	return no;

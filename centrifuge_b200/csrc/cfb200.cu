@@ -1114,26 +1114,68 @@ __global__ void __launch_bounds__(128, MINB) k_prep(const UnitArgs a) {
 	if(rows && off + rows <= a.rows_cap) { EmitRows er(a.p, u, a.rows + off); for_each_visit(a.p, u, er); }   // else: the host grows the buffer and re-runs EMIT_ONLY
 }
 
-static const int kLocalMap = 4;          // larger maps make every unit pay for a bigger local frame to spare the few heavy units their global scratch
+// k_prep hands out row slices per warp, so the rows of a warp's 32 units form one contiguous span.  A warp whose span fits
+// what is left of its CTA's pool stages the span's rows and ids there with coalesced loads; each unit keeps its hit map,
+// TaxCnt scratch and records at its own offset inside the span (nmap <= n bounds them), and the warp stores the records
+// coalesced.  A warp whose span does not fit uses the global scratch at the units' row offsets.
+static const int kScoreThreads = 128;
+static const uint32_t kScorePool = 128;       // rows per CTA, 116 bytes each (row, id, Entry, TaxCnt, OutRec); 256 made k_score faster but slowed e2e, where it shares SMs with search kernels (measured)
+static const uint32_t kNoSlot = 0xffffffffu;
 template <int MINB>
-__global__ void __launch_bounds__(128, MINB) k_score(const UnitArgs a) {
+__global__ void __launch_bounds__(kScoreThreads, MINB) k_score(const UnitArgs a) {
+	__shared__ uint64_t s_rows[kScorePool]; __shared__ uint32_t s_ids[kScorePool];
+	__shared__ Entry s_map[kScorePool]; __shared__ TaxCnt s_tc[kScorePool]; __shared__ OutRec s_recs[kScorePool];
+	__shared__ uint32_t s_used;
+	if(threadIdx.x == 0) s_used = 0;
+	__syncthreads();
 	const uint32_t unit = blockIdx.x * blockDim.x + threadIdx.x;
-	if(unit >= a.b.n_units) return;
+	const unsigned lane = threadIdx.x & 31;
+	const bool valid = unit < a.b.n_units;
+	const bool fits = *a.row_total <= a.rows_cap;          // else the host grows the row buffer and runs the batch's tail again
+	const uint64_t n = valid && fits ? a.nrows[unit] : 0, off = valid && fits ? a.row_off[unit] : 0;
+	const uint64_t base = __shfl_sync(0xffffffffu, off, 0);        // lane 0's unit is the warp's first: its slice starts the span
+	uint64_t span = n ? off + n - base : 0;
+	for(int d = 16; d > 0; d >>= 1) span = max(span, __shfl_xor_sync(0xffffffffu, span, d));
+	uint32_t slot = kNoSlot;
+	if(lane == 0 && span) {
+		uint32_t cur = *(volatile uint32_t*)&s_used;
+		while(span <= kScorePool - cur) {
+			const uint32_t old = atomicCAS(&s_used, cur, cur + (uint32_t)span);
+			if(old == cur) { slot = cur; break; }
+			cur = old;
+		}
+	}
+	slot = __shfl_sync(0xffffffffu, slot, 0);
+	const bool sh = slot != kNoSlot;
+	if(sh) {
+		for(uint32_t j = lane; j < (uint32_t)span; j += 32) { s_rows[slot + j] = a.rows[base + j]; s_ids[slot + j] = a.ids[base + j]; }
+		__syncwarp();
+	}
+	const uint32_t loc = sh ? slot + (uint32_t)(off - base) : 0u;
 	uint32_t no = 0;
-	const uint64_t off = a.row_off[unit], n = a.nrows[unit];
-	if(n > 0 && *a.row_total <= a.rows_cap) {
+	if(n > 0) {
 		const uint8_t fl = a.b.flags ? a.b.flags[unit] : 3;
 		int mates = 0;
 		for(int m = 0; m < a.b.n_mates; m++) if(((fl >> m) & 1) && (m ? a.b.len[1][unit] : a.b.len[0][unit]) != 0) mates++;
-		// the hit map of a unit with a handful of rows lives in thread-local memory (interleaved across the warp, L1-resident)
-		// instead of the per-unit slice of the global scratch, whose 72-byte entries of neighbouring threads never share a sector
-		Entry lmap[kLocalMap]; TaxCnt ltc[kLocalMap];
-		Entry* map = n <= (uint64_t)kLocalMap ? lmap : a.entries + off;
-		TaxCnt* tc = n <= (uint64_t)kLocalMap ? ltc : a.tcs + off;
-		const uint32_t nmap = score_plan(a.v, a.p, a.rows + off, a.ids + off, n, map);
-		no = reduce_and_emit(a.v, a.p, mates == 2, map, nmap, tc, a.recs_sparse + off);
+		const uint64_t* rows = sh ? s_rows + loc : a.rows + off;
+		const uint32_t* ids = sh ? s_ids + loc : a.ids + off;
+		Entry* map = sh ? s_map + loc : a.entries + off;
+		TaxCnt* tc = sh ? s_tc + loc : a.tcs + off;
+		OutRec* out = sh ? s_recs + loc : a.recs_sparse + off;
+		const uint32_t nmap = score_plan(a.v, a.p, rows, ids, n, map);
+		no = reduce_and_emit(a.v, a.p, mates == 2, map, nmap, tc, out);
 	}
-	a.nout[unit] = no;
+	if(valid) a.nout[unit] = no;
+	if(sh) {        // each unit's records, three 8-byte words apiece, stored by the whole warp
+		__syncwarp();
+		for(int u = 0; u < 32; u++) {
+			const uint32_t cnt = __shfl_sync(0xffffffffu, no, u) * 3u, l = __shfl_sync(0xffffffffu, loc, u);
+			const uint64_t o = __shfl_sync(0xffffffffu, off, u);
+			const uint64_t* src = reinterpret_cast<const uint64_t*>(s_recs + l);
+			uint64_t* dst = reinterpret_cast<uint64_t*>(a.recs_sparse + o);
+			for(uint32_t w = lane; w < cnt; w += 32) dst[w] = src[w];
+		}
+	}
 }
 
 // =======================================================================================
@@ -2235,7 +2277,7 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	else { if(c->count) k_resolve<true><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra); else k_resolve<false><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra); }
 	c->launches++;
 	if(time_it) CK(cudaEventRecord(s.ev[3], s.st));
-	k_score<12><<<ublocks, 128, 0, s.st>>>(ua); c->launches++;           // <= 40 registers: occupancy beats the few spills (measured)
+	k_score<12><<<ublocks, kScoreThreads, 0, s.st>>>(ua); c->launches++;        // <= 40 registers and 15.9 KB of shared memory: 12 CTAs per SM
 	k_scan_sums<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.nout.p, n, s.bsum.p);
 	k_scan_top<<<1, 1024, 0, s.st>>>(s.bsum.p, scan_blocks, (uint64_t*)(s.scal.p + 4));
 	k_scan_apply<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.nout.p, n, s.bsum.p, (const uint64_t*)(s.scal.p + 4), s.out_off.p);
