@@ -68,8 +68,8 @@ int cfb_index_get_info(const cfb_index*, cfb_index_info* out);
 /* What the device replica holds (bytes of HBM each; 0 = not built).  The derived tables are built at load time in
  * this order of benefit per byte, each only while it fits the budget left after the batch head-room (12 GB unless
  * CFB_HBM_HEADROOM_GB says otherwise; DESIGN.md 3): rank16 + ftab2 (always), the K-mer jump table (whose 16-byte entries
- * also carry the death bitmap), the resolve table, walk8 (possibly for a prefix of the rows).  The file's sides are dropped once rank16 exists (sides_bytes = 0)
- * except on small indexes, where the sides-based A/B kernels and test hooks stay usable. */
+ * also carry the death bitmap), the resolve table, walk8 (possibly for a prefix of the rows).  The file's sides only stage
+ * rank16 and are freed once it is built, so sides_bytes is always 0. */
 typedef struct {
 	uint64_t sides_bytes, sample_bytes, rank16_bytes, ftab2_bytes, ftabk_bytes, resolve_table_bytes, walk8_bytes;
 	uint64_t total_bytes, free_bytes_after_load;
@@ -264,7 +264,7 @@ int   cfb_device_count(void);         /* usable CUDA devices (0 without a driver
 void* cfb_host_alloc(size_t bytes);   /* pinned host memory (portable: every device of the process can DMA from it) */
 void  cfb_host_free(void*);
 
-/* Device unit-test hooks (tests/ only): run the cooperative LF / resolve primitives on
+/* Device unit-test hooks (tests/ only): run the product's LF and resolve walk on rank16 over
  * arrays of rows.  out[i] = LF(rows[i], chars[i]) ; chars[i] > 3 means BWT[rows[i]]. */
 int cfb_test_lf(const cfb_index*, const uint64_t* rows, const uint8_t* chars, uint64_t n, uint64_t* out);
 int cfb_test_resolve(const cfb_index*, const uint64_t* rows, uint64_t n, uint32_t* out);

@@ -49,8 +49,8 @@ def assert_same(on, orec, gn, grec):
         assert np.array_equal(orec[f], grec[f]), f
 
 
-def test_cooperative_lf_and_resolve_primitives(adv_base):
-    """8-lane side fetch + popcount rank + shuffle reduce == scalar LF of the oracle on random rows."""
+def test_rank16_lf_and_resolve_hooks(adv_base):
+    """The scalar LF and BWT[row] on rank16 (cf_logic.h, the extension step's LF) and k_resolve_c == the oracle on random rows."""
     import ctypes as C
     m = capi()
     ix = m.Index(adv_base, 0)
@@ -100,14 +100,13 @@ LAYOUT_VARIANTS = {
     "no_tables": {"CFB_WALK8": "0", "CFB_RESOLVE_TABLE": "0", "CFB_FTABK": "10", "CFB_FTABD": "0"},
     "ftabk11": {"CFB_FTABK": "11"},
     "ftabk12_walk_resolve": {"CFB_FTABK": "12", "CFB_RESOLVE_TABLE": "0"},
-    "coop8": {"CFB_GROUP": "8", "CFB_LEGACY_LAYOUTS": "1"},
     "tiny_row_buffer": {"CFB_ROWS_CAP": "64"},          # every batch overflows the row buffer once and re-runs from the row stage
 }
 
 
 @pytest.mark.parametrize("variant", sorted(LAYOUT_VARIANTS))
 def test_every_device_layout_gives_the_same_records(variant, adv_base, adv_reads, monkeypatch):
-    """The derived tables (K-mer jump table, resolve table, walk8) and the kernel variants are pure
+    """The derived tables (K-mer jump table, resolve table, walk8) and the search options are pure
     accelerations: with any of them switched off the records are the oracle's as well."""
     for k, v in LAYOUT_VARIANTS[variant].items():
         monkeypatch.setenv(k, v)

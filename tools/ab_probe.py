@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """One classification of N bench reads on the bench index under whatever CFB_* knobs the environment sets -- the
-unit of an ncu A/B capture (e.g. CFB_GROUP=8 CFB_KEEP_SIDES=1 for the warp-cooperative kernel of the north-star
-design next to the default thread-per-walk kernel).  usage: ab_probe.py [n_reads]"""
+unit of an ncu A/B capture (e.g. CFB_WALK8=0 for the search without walk8 next to the default tables).
+usage: ab_probe.py [n_reads]"""
 import os
 import sys
 import time
