@@ -319,6 +319,13 @@ class Context:
         _ck(lib().cfb_ctx_requests(self.h, out))
         return dict(zip(["rank16", "ftab2", "ftabk", "walk8", "ftabd"], [int(x) for x in out]))
 
+    def request_breakdown(self):
+        """where the CFB_COUNT=2 requests of the last batch go: rank16 requests by range width, walk8 jumps tried / taken"""
+        out = (C.c_uint64 * 8)()
+        _ck(lib().cfb_ctx_request_breakdown(self.h, out))
+        names = ["rank16_w1", "rank16_w2_4", "rank16_w5", "walk8_try_row", "walk8_ok_row", "walk8_try_range", "walk8_ok_range", "walk8_ok_w5"]
+        return dict(zip(names, [int(x) for x in out]))
+
     def counters(self):
         out = (C.c_uint64 * 8)()
         _ck(lib().cfb_ctx_counters(self.h, out))

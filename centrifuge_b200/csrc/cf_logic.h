@@ -81,6 +81,9 @@ struct Counters {   // algorithmic-operation counters (SURVEY.md section 8d defi
 	// rank16 entries (16 B), 10-mer table entries (16 B), K-mer table entries (16 B), walk8 entries (8 B); req_ftabd stays 0
 	// (the death bitmap is read with the K-mer table entry)
 	unsigned long long req_rank16, req_ftab2, req_ftabk, req_walk8, req_ftabd;
+	// where the requests of count mode 2 go: rank16 requests made while the range has width 1, 2-4 and >= 5 (they sum to
+	// req_rank16), and walk8 jumps tried and taken from a single row and from a range (w8_ok_w5: taken from width >= 5)
+	unsigned long long r16_w1, r16_w2_4, r16_w5, w8_try_row, w8_ok_row, w8_try_range, w8_ok_range, w8_ok_w5;
 };
 
 CFB_HD int popc64(uint64_t x) {
@@ -89,6 +92,36 @@ CFB_HD int popc64(uint64_t x) {
 #else
 	return __builtin_popcountll(x);
 #endif
+}
+CFB_HD uint32_t ctz32(uint32_t x) {      // x != 0
+#ifdef __CUDA_ARCH__
+	return (uint32_t)(__ffs(x) - 1);
+#else
+	return (uint32_t)__builtin_ctz(x);
+#endif
+}
+
+// walk8 (k_build_walk8): per SA row r, the row eight successive mapLF1 steps reach (bits 0-39), the eight BWT bases met on the
+// way (2 bits each from bit 40, first step lowest) and the number of valid steps (bits 56-63; fewer than 8 when the walk meets
+// the '$' row).  walk8_steps = how many of the next eight read bases (`win`: 2 bits each, base p in bits 2p; N bits in `nwin`)
+// row r follows: 8 = all of them, else the step at which it leaves the range (a different base, an N, or the '$' row).
+//
+// Range rule.  The range of cP is the set of LF images of the rows of P's range [top, bot) whose BWT base is c; LF keeps
+// their order, so when top and bot - 1 both have base c the new range is exactly [LF(top), LF(bot - 1) + 1), whatever the
+// rows between them do.  By induction: when both end rows follow all eight bases, the range after them is exactly
+// [W8(top), W8(bot - 1) + 1) -- possibly narrower (interior rows may drop out), never empty.  And an end row stays the end
+// of the range for as long as it follows the read, so after a failed attempt every jump tried before both failing ends have
+// left fails the same way: walk8_retry is the first step from which the next attempt can succeed.
+static const uint64_t kWalkRowMask = (1ull << 40) - 1ull;
+CFB_HD uint32_t walk8_steps(uint64_t e, uint64_t win, uint32_t nwin) {
+	const uint32_t diff = (uint32_t)(((e >> 40) ^ win) & 0xffffull), nb = nwin & 0xffu, nv = (uint32_t)(e >> 56);
+	uint32_t good = diff ? ctz32(diff) >> 1 : 8u;
+	if(nb) { const uint32_t n = ctz32(nb); good = n < good ? n : good; }
+	return nv < good ? nv : good;
+}
+CFB_HD uint32_t walk8_retry(uint32_t st, uint32_t sb) {     // steps of the two end rows, at least one below 8
+	const uint32_t a = st < 8u ? st : 0u, b = sb < 8u ? sb : 0u;
+	return (a > b ? a : b) + 1u;
 }
 
 // positions (bit 2i) where the 2-bit code at i equals c

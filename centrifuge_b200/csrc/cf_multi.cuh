@@ -187,6 +187,14 @@ extern "C" int cfb_ctx_requests(cfb_ctx* c, uint64_t out[5]) {
 	out[0] = h.req_rank16; out[1] = h.req_ftab2; out[2] = h.req_ftabk; out[3] = h.req_walk8; out[4] = h.req_ftabd;
 	return CFB_OK;
 }
+extern "C" int cfb_ctx_request_breakdown(cfb_ctx* c, uint64_t out[8]) {
+	if(!c || !out) return fail(CFB_EINVAL, "null argument");
+	CK(cudaSetDevice(c->ix->device));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	out[0] = h.r16_w1; out[1] = h.r16_w2_4; out[2] = h.r16_w5;
+	out[3] = h.w8_try_row; out[4] = h.w8_ok_row; out[5] = h.w8_try_range; out[6] = h.w8_ok_range; out[7] = h.w8_ok_w5;
+	return CFB_OK;
+}
 
 __device__ __forceinline__ uint64_t gmix(uint64_t x) { x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31); }
 // independent, uniformly random gathers of W 8-byte words per request from array `a` of `n` requests' worth, `iters` x ILP per thread

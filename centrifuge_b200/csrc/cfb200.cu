@@ -31,7 +31,7 @@ struct SearchArgs {
 	unsigned int* overflow;
 	Counters* ctr;
 	const uint64_t* pk; const uint32_t* nm; uint32_t W;   // packed reads (k_pack)
-	uint32_t jump_w;                                      // widest range advanced eight bases per gather through walk8 (CFB_JUMP_W, default 4)
+	uint32_t jump_w;                                      // widest range k_search_t advances eight bases per walk8 gather (CFB_JUMP_W; default: any width)
 	uint32_t keep_short;                                  // store every hit (min_hitlen < 22, k_search_long); else only hits of >= kLongLen bases
 };
 
@@ -198,7 +198,6 @@ __host__ __device__ __forceinline__ uint32_t nh_pack(uint32_t stored, uint32_t f
 __host__ __device__ __forceinline__ uint32_t nh_stored(uint32_t w) { return w & 0x7fffu; }
 __host__ __device__ __forceinline__ uint32_t nh_found(uint32_t w) { return (w >> 15) & 0x7fffu; }
 static const uint64_t kOccMask = 0x7fffffffffffffffull;
-static const uint64_t kWalkRowMask = (1ull << 40) - 1ull;   // walk8 entry: row in the low 40 bits
 
 // K-mer jump table: one 16-byte entry per K-mer (K >= ftabChars) that a partial search gathers in place of its first K
 // steps (hi_aligner.h:985-1008), trading HBM capacity (16 B x 4^K; 17 GB at K = 15) for random accesses.
@@ -310,10 +309,11 @@ template <int RW> struct ReadRegs {
 // COUNT: 0 = product; 1 = the reference's operation counters (SURVEY 8d: jump tables off, so that the operation sequence is the
 // reference's); 2 = the product's own load requests with every table live (what the roofline of *this* kernel is made of)
 template <int COUNT, int RW>
-__global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a) {
-	// RW = 4: 58 registers, 8 CTAs per SM.  Forcing 9 (__launch_bounds__(kSearchThreads, 9): 56 registers, no spills) took the
-	// search kernel from 28.0 to 27.4 ms per 10 M reads on one H100 80GB HBM3 at 400 W, but reads/s moved by about one
-	// run-to-run spread (256.4 vs 259.7 M, three runs each), so it is not forced: the DRAM gather rate is the limit
+__global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1) k_search_t(const SearchArgs a) {
+	// RW = 4: 56 registers, 8 CTAs per SM; RW = 5 keeps 8 CTAs through the launch bounds (62 registers, no spills).  Forcing 9
+	// for RW = 4 (then at 58 registers; 56 with the bound, no spills) took the search kernel from 28.0 to 27.4 ms per 10 M reads on
+	// one H100 80GB HBM3 at 400 W, but reads/s moved by about one run-to-run spread (256.4 vs 259.7 M, three runs each), so it is
+	// not forced: the DRAM gather rate is the limit
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(a.v.rank16);
 	const ulonglong2* ftab2 = reinterpret_cast<const ulonglong2*>(a.v.ftab2);
 	const ulonglong2* ftabk = reinterpret_cast<const ulonglong2*>(a.v.ftabk);
@@ -325,11 +325,12 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a)
 	const uint32_t fd = (fk == 0 || a.p.min_hitlen < (uint32_t)a.v.ftabd_chars) ? 0u : (uint32_t)a.v.ftabd_chars;
 	ReadRegs<RW> rd;
 	uint64_t top = 0, bot = 0, fi = 0;      // M_FTABK: fi = K-mer | (64 | extension) << 2K when the bitmap applies
-	uint32_t rlen = 0, tid = 0, cur = 0, dep = 0, offset = 0, nh = 0, nt = 0, slow_until = 0, fail_w = 0, fail_at = 0xffffffffu;
+	uint32_t rlen = 0, tid = 0, cur = 0, dep = 0, offset = 0, nh = 0, nt = 0, slow_until = 0, fail_at = 0xffffffffu;
 	bool nolong = true;      // no hit of this strand reaches min_hitlen (kListNoLong tells the per-unit kernels)
 	int mode = M_NEED;
 	unsigned long long c_ps = 0, c_ft = 0, c_sides = 0, c_lf = 0;
 	unsigned long long q_r16 = 0, q_f2 = 0, q_fk = 0, q_w8 = 0;
+	unsigned long long q_w1 = 0, q_w24 = 0, q_w5 = 0, j_row = 0, j_row_ok = 0, j_rng = 0, j_rng_ok = 0, j_w5_ok = 0;
 	WarpPool pool; pool.base = pool.end = 0;
 	bool more = true;      // warp-uniform: the global task counter is not exhausted yet
 
@@ -397,7 +398,7 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a)
 						const uint8_t fl = a.b.flags ? a.b.flags[unit] : 3;
 						nh = 0; nt = 0; rlen = a.b.len[mate][unit];
 						if(!((fl >> mate) & 1) || rlen == 0) a.nhits[tid] = 0;          // filtered mate: stays M_NEED
-						else { rd.load(a.pk + (size_t)tid * a.W, a.nm + (size_t)tid * a.W, a.W); cur = 0; slow_until = 0; fail_w = 0; fail_at = 0xffffffffu; nolong = true; start_search(); }
+						else { rd.load(a.pk + (size_t)tid * a.W, a.nm + (size_t)tid * a.W, a.W); cur = 0; slow_until = 0; fail_at = 0xffffffffu; nolong = true; start_search(); }
 					} else mode = M_DONE;
 				}
 				if(__any_sync(0xffffffffu, want && !got)) more = false;      // global counter ran past the end
@@ -422,17 +423,17 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a)
 				range = (bot - top) != 1;
 				const uint64_t width = bot - top;
 				if(dep == fail_at && !range) known_fail = true;      // the walk8 entry already said that this step of the single row fails: no request
-				else if(w8 && width <= (uint64_t)a.jump_w && (dep >= slow_until || width < (uint64_t)fail_w) && rlen - dep >= 8 && bot <= a.v.walk8_rows) {
-					// Eight steps in one gather: while the walk holds a single row -- or a narrow range -- and the read's next eight
-					// bases are the ones stored for its first AND its last row.  LF keeps the order of rows that continue with the
-					// same base, so the range survives the eight steps intact exactly when both end rows do and their images are
-					// still width - 1 apart (every row that drops out in between shortens that distance by one, nothing widens it).
-					jump = true; p0 = w8 + (top & ~1ull); sub = (uint32_t)(top & 1); if(COUNT == 2) q_w8++;
-					if(range) { const uint64_t last = bot - 1; sub |= (uint32_t)(last & 1) << 1; if((last & ~1ull) != (top & ~1ull)) { p1 = w8 + (last & ~1ull); if(COUNT == 2) q_w8++; } }
+				else if(w8 && width <= (uint64_t)a.jump_w && dep >= slow_until && rlen - dep >= 8 && bot <= a.v.walk8_rows) {
+					// Eight steps in one gather: the read's next eight bases are the ones stored for the range's first AND last
+					// row.  Then the range after them is exactly [W8(top), W8(bot - 1) + 1), whatever the rows in between do
+					// (cf_logic.h, walk8_steps).  One 16-byte piece serves both ends when they share it.
+					jump = true; p0 = w8 + (top & ~1ull); sub = (uint32_t)(top & 1);
+					if(range) { const uint64_t last = bot - 1; sub |= (uint32_t)(last & 1) << 1; if((last & ~1ull) != (top & ~1ull)) p1 = w8 + (last & ~1ull); }
+					if(COUNT == 2) { q_w8 += p1 ? 2 : 1; if(range) j_rng++; else j_row++; }
 				} else {
 					p0 = r16 + (top >> 6) * 4 + c;                          // (occ, bits): one request per rank query
-					if(COUNT == 2) q_r16++;
-					if(range && (bot >> 6) != (top >> 6)) { p1 = r16 + (bot >> 6) * 4 + c; if(COUNT == 2) q_r16++; }
+					if(range && (bot >> 6) != (top >> 6)) p1 = r16 + (bot >> 6) * 4 + c;
+					if(COUNT == 2) { const uint32_t n = p1 ? 2 : 1; q_r16 += n; if(width == 1) q_w1 += n; else if(width <= 4) q_w24 += n; else q_w5 += n; }
 				}
 			}
 		}
@@ -469,21 +470,15 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a)
 		} else if(jump) {
 			uint64_t win; uint32_t nwin; rd.window(dep, win, nwin);
 			const uint64_t w = (sub & 1u) ? e.y : e.x;                       // entry of the first row
-			const uint64_t wl = (sub & 2u) ? bq.y : bq.x;                    // entry of the last row (the same entry for a single row)
-			const uint64_t width = bot - top;
-			if((w >> 56) == 8 && !(nwin & 0xffu) && !(((w >> 40) ^ win) & 0xffffull)
-			   && (width == 1 || ((wl >> 40) == (w >> 40) && (wl & kWalkRowMask) - (w & kWalkRowMask) == width - 1))) {
-				top = w & kWalkRowMask; bot = top + width; dep += 8;
+			const uint64_t wl = range ? ((sub & 2u) ? bq.y : bq.x) : w;      // entry of the last row
+			const uint32_t st = walk8_steps(w, win, nwin), sb = range ? walk8_steps(wl, win, nwin) : st;
+			if((st & sb) == 8u) {                                            // both end rows follow all eight bases
+				if(COUNT == 2) { if(range) j_rng_ok++; else j_row_ok++; if(bot - top >= 5) j_w5_ok++; }
+				top = w & kWalkRowMask; bot = (wl & kWalkRowMask) + 1; dep += 8;
 				if(dep >= rlen) hit_and_restart();
-			} else {      // some row leaves within the next eight steps: take them one by one (a narrower range may try again)
-				slow_until = dep + 8; fail_w = (uint32_t)width;
-				if(width == 1) {      // a single row: the entry tells which step ends the hit (first stored base that differs, an N, or the '$' row)
-					const uint32_t diff = (uint32_t)(((w >> 40) ^ win) & 0xffffull), nb = nwin & 0xffu, nv = (uint32_t)(w >> 56) & 0xffu;
-					uint32_t good = diff ? (uint32_t)(__ffs(diff) - 1) >> 1 : 8u;
-					if(nb) good = min(good, (uint32_t)(__ffs(nb) - 1));
-					good = min(good, nv);
-					fail_at = good < 8u ? dep + good : 0xffffffffu;
-				}
+			} else {      // an end row leaves within the next eight steps: take them one by one until both failing ends have left
+				slow_until = dep + walk8_retry(st, sb);
+				if(!range) fail_at = dep + st;      // a single row: the entry tells which step ends the hit (no request for it)
 			}
 		} else if(lf) {
 			bool fail = c > 3 || known_fail;
@@ -513,6 +508,8 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_t(const SearchArgs a)
 	}
 	if(COUNT == 2 && a.ctr) {
 		atomicAdd(&a.ctr->req_rank16, q_r16); atomicAdd(&a.ctr->req_ftab2, q_f2); atomicAdd(&a.ctr->req_ftabk, q_fk); atomicAdd(&a.ctr->req_walk8, q_w8);
+		atomicAdd(&a.ctr->r16_w1, q_w1); atomicAdd(&a.ctr->r16_w2_4, q_w24); atomicAdd(&a.ctr->r16_w5, q_w5);
+		atomicAdd(&a.ctr->w8_try_row, j_row); atomicAdd(&a.ctr->w8_ok_row, j_row_ok); atomicAdd(&a.ctr->w8_try_range, j_rng); atomicAdd(&a.ctr->w8_ok_range, j_rng_ok); atomicAdd(&a.ctr->w8_ok_w5, j_w5_ok);
 	}
 }
 
@@ -534,7 +531,7 @@ struct UnitArgs {
 
 // One strand's whole greedy search by a single thread, with the device tables: the hits search_strand_scalar (cf_logic.h, the
 // twin the CPU tests pin against the oracle) would produce, but reached the way k_search_t reaches them -- K-mer jump, one
-// rank16 entry per step when top and bot share a block, eight bases per walk8 gather on a single row -- so that regenerating
+// rank16 entry per step when top and bot share a block, eight bases per walk8 gather of the range's end rows -- so that regenerating
 // a list costs ~30 dependent gathers instead of ~250.  Used by k_prep (lists whose short hits matter) and k_search_long.
 __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t len, int strand, HitRec* hits, uint32_t cap) {
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(v.rank16);
@@ -562,16 +559,19 @@ __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const
 				if(!have) { const ulonglong2 e = __ldg(ftab2 + (fi & ((1ull << (2 * fc)) - 1ull))); top = e.x; bot = e.y; dep = cur + fc; }
 				if(bot <= top) { h.top = h.bot = kOff; h.len = dep - offset; new_cur = dep; done = dep >= len; }
 				else {
+					uint32_t slow_until = 0;
 					while(dep < len) {
 						const int c = base(dep);
 						if(c > 3) break;
+						if(v.walk8 && bot <= v.walk8_rows && len - dep >= 8 && dep >= slow_until) {     // eight bases in one gather (k_search_t's rule)
+							uint64_t win = 0; uint32_t nwin = 0;
+							for(uint32_t j = 0; j < 8; j++) { const int b = base(dep + j); if(b > 3) nwin |= 1u << j; else win |= (uint64_t)b << (2 * j); }
+							const uint64_t et = __ldg(v.walk8 + top), eb = bot - top == 1 ? et : __ldg(v.walk8 + bot - 1);
+							const uint32_t st = walk8_steps(et, win, nwin), sb = walk8_steps(eb, win, nwin);
+							if((st & sb) == 8u) { top = et & kWalkRowMask; bot = (eb & kWalkRowMask) + 1; dep += 8; continue; }
+							slow_until = dep + walk8_retry(st, sb);
+						}
 						if(bot - top == 1) {
-							if(v.walk8 && top < v.walk8_rows && len - dep >= 8) {        // eight bases in one gather
-								const uint64_t e = __ldg(v.walk8 + top);
-								bool ok = (e >> 56) == 8;
-								for(uint32_t j = 0; ok && j < 8; j++) ok = base(dep + j) == (int)((e >> (40 + 2 * j)) & 3);
-								if(ok) { top = e & kWalkRowMask; bot = top + 1; dep += 8; continue; }
-							}
 							const ulonglong2 e = __ldg(r16 + (top >> 6) * 4 + c);
 							if(!((e.y >> (top & 63)) & 1ull)) break;                      // mapLF1: BWT[top] must be c ('$' has no bit)
 							top = v.fchr[c] + (e.x & kOccMask) + (uint64_t)__popcll(e.y & ((1ull << (top & 63)) - 1ull)); bot = top + 1; dep++;
@@ -1133,7 +1133,9 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 			// 80 GB H100: 4 slots of 0.5 M 100 bp reads in flight at ~3 KB each with 30 % to grow,
 			// plus 3 GB of fixed buffers; callers that keep more in flight set CFB_HBM_HEADROOM_GB, as bench.py does).  Tables are built in the order of gathers saved per
 			// byte -- K-mer jump table, resolve table, walk8 -- each only if it fits what is left; walk8, whose rows are hit
-			// uniformly, may cover just a prefix of the rows (a jump needs an entry for the row it starts from only).
+			// uniformly, may cover just a prefix of the rows (a jump needs the entries of the range's two end rows only).  With
+			// range jumps, K = 14 (4.3 GB, walk8 on 34 % of the bench index's rows instead of 16 %) measured the same as K = 15
+			// (274.5 vs 274.6-275.7 M reads/s on one H100 80GB HBM3 at 400 W), so the K-mer table keeps its place in the order.
 			size_t free_b = 0, total_b = 0; cudaMemGetInfo(&free_b, &total_b);
 			double head_gb = 12.0; { const char* e = getenv("CFB_HBM_HEADROOM_GB"); if(e) head_gb = atof(e); }
 			const uint64_t headroom = std::min<uint64_t>((uint64_t)(head_gb * 1073741824.0), free_b / 2);
@@ -1308,7 +1310,7 @@ struct cfb_ctx {
 	uint64_t rows_cap0 = 0;       // CFB_ROWS_CAP: initial row-buffer capacity (tests force the grow-and-re-run path with it)
 	TextCtx* text = nullptr;
 	CountsCtx cnt; bool fold_records = false;
-	uint32_t jump_w = 4; bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
+	uint32_t jump_w = 0xffffffffu; bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
 	uint64_t regen_lists = 0, regen_tasks = 0;   // lists regenerated / strand lists searched so far (CFB_REGEN_STATS=1 prints them when the context goes)
 	uint64_t regen_slots0 = 0;    // CFB_REGEN_SLOTS: initial capacity of the list-regeneration buffer (tests force the grow-and-re-run path with it)
 	void* comm = nullptr; int comm_rank = 0, comm_size = 1; cudaStream_t comm_st = nullptr;      // NCCL communicator (cf_multi.cuh)
@@ -1402,7 +1404,7 @@ extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx*
 	{ const char* rc0 = getenv("CFB_ROWS_CAP"); if(rc0) c->rows_cap0 = strtoull(rc0, NULL, 10); }
 	{ const char* ks = getenv("CFB_KEEP_SHORT"); c->keep_short = ks && ks[0] == '1'; }
 	{ const char* rs = getenv("CFB_REGEN_SLOTS"); if(rs) c->regen_slots0 = strtoull(rs, NULL, 10); }
-	{ const char* jw = getenv("CFB_JUMP_W"); c->jump_w = jw ? (uint32_t)std::min(std::max(atoi(jw), 1), 8) : 4u; }      // 1..8; wider jumps save dependent gathers
+	{ const char* jw = getenv("CFB_JUMP_W"); c->jump_w = jw && atoi(jw) > 0 ? (uint32_t)atoi(jw) : 0xffffffffu; }      // A/B cap on the range width of a walk8 jump (unset or 0: any width)
 	const char* cnt = getenv("CFB_COUNT");
 	c->count = cnt ? (cnt[0] == '1' ? 1 : (cnt[0] == '2' ? 2 : 0)) : 0;
 	#undef CKC

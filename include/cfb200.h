@@ -253,6 +253,10 @@ int cfb_counts_allreduce(cfb_ctx* const* ctxs, int n, uint64_t* dense_out, uint6
  * ceiling of this device over the replica's own arrays: independent uniformly random gathers from table 0 = rank16
  * (16 B), 1 = K-mer table (16 B), 2 = walk8 (8 B), 3 = resolve table (8 B), in G requests/s; 4 (death bits: no table of their own) always fails as not built. */
 int cfb_ctx_requests(cfb_ctx*, uint64_t out[5]);
+/* Where those requests go (CFB_COUNT=2): {rank16 requests made while the range has width 1, width 2-4, width >= 5 (the three sum
+ * to the rank16 entries above), walk8 jumps tried from a single row, taken from a single row, tried from a range, taken from a
+ * range, taken from a range of width >= 5}.  A separate call, so that the sum of cfb_ctx_requests stays the total request count. */
+int cfb_ctx_request_breakdown(cfb_ctx*, uint64_t out[8]);
 int cfb_gather_ceiling(const cfb_index*, int table, uint64_t n_requests, double* g_requests_per_s, double* ms);
 
 /* Operation counters of the last batch on this ctx (same definition as SURVEY.md 8d):
