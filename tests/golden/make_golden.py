@@ -4,6 +4,7 @@ oracle/_ref (built from the reference sources by `make -C oracle ref`).  Run wit
 outputs are committed so that the oracle stays pinned where the reference is not available.
 
   adv.{1,2,3,4}.cf.xz   index of tools/synth.py:write_adversarial (seed 33) built by centrifuge-build-bin
+  adv_t<T>o<O>.{1,2,3,4}.cf.xz   the same genomes built with -t/--ftabchars T and -o/--offrate O (GEOMETRIES below)
   adv.reads.fa.xz       its reads
   adv.<case>.tsv.xz / adv.<case>.report.tsv   centrifuge-class output per option set (CASES below)
   example.*             output of the reference's own example fixture (MANUAL.markdown:1586-1603)
@@ -31,6 +32,9 @@ CASES = {
     "family": ["--classification-rank", "family"],
     "notraverse": ["--no-traverse"],
 }
+# (ftabChars, offRate) of the other committed builds of the adv genomes: every sampled row (-o 0), the smallest ftab (-t 1)
+# and long resolve walks (-o 7).  -t 12 is not committed (its ftab alone is 134 MB): tests build it and check its digest.
+GEOMETRIES = {"adv_t6o0": (6, 0), "adv_t1o2": (1, 2), "adv_t8o7": (8, 7)}
 
 
 def xz(src, dst):
@@ -47,6 +51,14 @@ def main():
                            os.path.join(tmp, "genomes.fa"), base], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
     for k in "1234":
         xz("%s.%s.cf" % (base, k), os.path.join(HERE, "adv.%s.cf.xz" % k))
+    for name, (t, o) in GEOMETRIES.items():
+        gbase = os.path.join(tmp, name)
+        subprocess.check_call([os.path.join(REF, "centrifuge-build-bin"), "-p", "4", "-t", str(t), "-o", str(o),
+                               "--conversion-table", os.path.join(tmp, "conv.tsv"), "--taxonomy-tree", os.path.join(tmp, "nodes.dmp"),
+                               "--name-table", os.path.join(tmp, "names.dmp"), os.path.join(tmp, "genomes.fa"), gbase],
+                              stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+        for k in "1234":
+            xz("%s.%s.cf" % (gbase, k), os.path.join(HERE, "%s.%s.cf.xz" % (name, k)))
     xz(os.path.join(tmp, "reads.fa"), os.path.join(HERE, "adv.reads.fa.xz"))
     for name, opts in CASES.items():
         out, rep = os.path.join(tmp, name + ".tsv"), os.path.join(tmp, name + ".rep")

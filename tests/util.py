@@ -119,20 +119,26 @@ def ref_script(name, tmp):
     return os.path.join(stage, name)
 
 
-def build_cf(fastas, conv, nodes, names, base, key):
+def geometry_args(ftab_chars=10, off_rate=4):
+    """centrifuge-build's -t/--ftabchars and -o/--offrate for an index geometry; none for the default (10, 4)."""
+    return ([] if ftab_chars == 10 else ["-t", str(ftab_chars)]) + ([] if off_rate == 4 else ["-o", str(off_rate)])
+
+
+def build_cf(fastas, conv, nodes, names, base, key, ftab_chars=10, off_rate=4):
     """.cf index of the FASTA files: built by the unmodified reference builder when recording, else by the project's own
     GPU builder (cfb_build_index), whose files must equal the reference's (compared by their recorded digest)."""
     def files():
         return [open("%s.%s.cf" % (base, k), "rb").read() for k in "1234"]
 
     def ref():
-        subprocess.check_call([REF_BUILD, "-p", "4", "--conversion-table", conv, "--taxonomy-tree", nodes, "--name-table", names,
-                               ",".join(fastas), base], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
+        subprocess.check_call([REF_BUILD, "-p", "4", "--conversion-table", conv, "--taxonomy-tree", nodes, "--name-table", names]
+                              + geometry_args(ftab_chars, off_rate) + [",".join(fastas), base], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
         return files()
     want = reference("index/" + key, ref)
     if not RECORD:
         from centrifuge_b200 import capi
-        capi.build_index(capi.build_opts(base, fasta=list(fastas), conversion_table=conv, taxonomy_tree=nodes, name_table=names))
+        capi.build_index(capi.build_opts(base, fasta=list(fastas), conversion_table=conv, taxonomy_tree=nodes, name_table=names,
+                                         ftab_chars=ftab_chars, off_rate=off_rate))
         if digest(files()) != want:
             raise AssertionError("index %s: the project's builder did not write the reference builder's bytes" % key)
 
@@ -152,16 +158,23 @@ def ensure_oracle():
 
 
 # ----------------------------------------------------------------------------- fixtures
-def build_index(tag, genera, species, length, seed, div=0.03, cid=False, strains=False):
-    """Synthetic genomes -> .cf index with the reference builder's bytes (build_cf).  Cached."""
-    key = hashlib.md5(repr((tag, genera, species, length, seed, div, cid, strains, ())).encode()).hexdigest()[:12]
-    d = os.path.join(CACHE, "%s_%s" % (tag, key))
+def index_key(tag, genera, species, length, seed, div=0.03, cid=False, strains=False, ftab_chars=10, off_rate=4):
+    """Cache directory name of build_index's index, and its recorded digest's key (index/<key>)."""
+    args = (tag, genera, species, length, seed, div, cid, strains, tuple(geometry_args(ftab_chars, off_rate)))
+    return "%s_%s" % (tag, hashlib.md5(repr(args).encode()).hexdigest()[:12])
+
+
+def build_index(tag, genera, species, length, seed, div=0.03, cid=False, strains=False, ftab_chars=10, off_rate=4):
+    """Synthetic genomes -> .cf index with the reference builder's bytes (build_cf).  Cached.  The builder arguments of a
+    non-default geometry go into the key's last field, so the default geometry keeps its key."""
+    key = index_key(tag, genera, species, length, seed, div, cid, strains, ftab_chars, off_rate)
+    d = os.path.join(CACHE, key)
     base = os.path.join(d, "idx")
     if not os.path.exists(os.path.join(d, "done")):
         os.makedirs(d, exist_ok=True)
         synth.write_genomes(d, genera, species, length, seed, div, cid, strains)
         build_cf([os.path.join(d, "genomes.fa")], os.path.join(d, "conv.tsv"), os.path.join(d, "nodes.dmp"), os.path.join(d, "names.dmp"),
-                 base, "%s_%s" % (tag, key))
+                 base, key, ftab_chars, off_rate)
         open(os.path.join(d, "done"), "w").close()
     return base
 
