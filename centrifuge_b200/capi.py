@@ -257,6 +257,11 @@ class Context:
         _ck(lib().cfb_resident_result(self.h, C.byref(res)))
         return _result(res)
 
+    def set_columns(self, cols=None):
+        """Columns of the rows of later text_submit calls: a --tab-fmt-cols list ("readID,taxID,readSeq,..."); None = the
+        default list.  An unknown name raises CfbError with the reference's message."""
+        _ck(lib().cfb_ctx_set_columns(self.h, cols.encode() if cols is not None else None))
+
     def text_submit(self, slot, text_a, text_b=None, n_records=0, fasta=False, trim5=0, trim3=0, seed=0, maxlen_hint=0):
         """text_a/text_b: uint8 arrays of complete records (pinned arrays are DMA'd in place)."""
         o = TextOpts(1 if fasta else 0, trim5, trim3, seed, maxlen_hint)

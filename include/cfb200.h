@@ -214,6 +214,13 @@ int cfb_text_submit(cfb_ctx*, int slot, const void* text_a, uint64_t bytes_a, co
                     uint64_t n_records, const cfb_text_opts*);
 /* discard != 0: drop the span's contribution to the per-taxon counters (the caller re-does it). */
 int cfb_text_wait(cfb_ctx*, int slot, int discard, cfb_text_result* out);
+/* Columns of the rows of later cfb_text_submit calls on this context: a `centrifuge-class --tab-fmt-cols` list (comma
+ * separated names; readID, seqID, taxID, taxRank/taxLevel, taxName, score, 2ndBestScore, hitLength, queryLength,
+ * numMatches, readSeq, readQual, readSeq1/SEQ1, readSeq2/SEQ2, readQual1/QUAL1, readQual2/QUAL2 and the SAM names
+ * QNAME, FLAG, RNAME, POS, MAPQ, CIGAR, RNEXT, PNEXT, TLEN, SEQ, QUAL), at most 64 of them.  NULL = the default list
+ * readID,seqID,taxID,score,2ndBestScore,hitLength,queryLength,numMatches.  Rows carry no header line.  An unknown name
+ * returns CFB_EINVAL with "Column definition <name> invalid." in cfb_last_error(). */
+int cfb_ctx_set_columns(cfb_ctx*, const char* cols);
 /* Per-taxon counters accumulated on the device by all accepted spans: entries with n_reads > 0.
  * n_obs1 = reads whose single best row reached the maximum score (observed keys of size 1). */
 int cfb_text_species(cfb_ctx*, uint64_t* taxid, uint64_t* n_reads, uint64_t* n_unique, uint64_t* n_obs1, uint64_t cap, uint64_t* n);
