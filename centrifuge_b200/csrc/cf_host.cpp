@@ -375,6 +375,9 @@ static void calc_abundance(const HostIndex& h, Species& sp, size_t& iters, doubl
 	// large problems (or CFB_GPU_EM=1) iterate on the device: same operations in the same order, same doubles
 	const char* ge = getenv("CFB_GPU_EM");
 	const bool on_device = device >= 0 && !p.empty() && ((ge && ge[0] == '1') || (!(ge && ge[0] == '0') && f.target.size() >= (1u << 18)));
+	if(getenv("CFB_TEXT_STATS"))
+		std::cerr << "[cfb] abundance EM: " << p.size() << " species, " << f.count.size() << " keys, " << f.target.size() << " contributions, on the "
+		          << (on_device ? "device" : "host") << std::endl;
 	size_t it = 0; double diff = 0.0;
 	if(on_device) {
 		uint64_t iters64 = 0;

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import util
+from util_em import em_lines_of, run_class
 
 pytestmark = pytest.mark.gpu
 
@@ -149,10 +150,16 @@ def test_two_gpu_cli_output_is_byte_identical_to_one_gpu(syn, tmp_path):
         assert p.returncode == 0, p.stderr.decode()
         if tag != "one":
             assert b"devices, per-taxon counters reduced with NCCL" in p.stderr
-        outs.append(tuple(open(str(tmp_path / (tag + ext)), "rb").read() for ext in (".tsv", ".rep", ".kr")))
+        outs.append(tuple(open(str(tmp_path / (tag + ext)), "rb").read() for ext in (".tsv", ".rep", ".kr")) + (em_lines_of(p.stderr),))
     assert outs[0] == outs[1] == outs[2]
     util.assert_matches(outs[1][:2], util.reference("gpu_multi/one_u_file", lambda: util.run_cli(
         util.REF_CLASS, ["-q", "-x", base, "-U", fq], str(tmp_path / "ref.tsv"), str(tmp_path / "ref.rep"))))
+    util.assert_matches(outs[1][3], reference_em_lines_one_u_file(base, fq, tmp_path))
+
+
+def reference_em_lines_one_u_file(base, fq, tmp):
+    """The reference binary's two EM lines on the reads of the two-GPU test (recorded, util.reference)."""
+    return util.reference("em/gpu_multi/one_u_file", lambda: run_class(util.REF_CLASS, ["-q", "-x", base, "-U", fq], tmp)[1])
 
 
 @pytest.mark.skipif(n_devices() < 2, reason="needs two GPUs")

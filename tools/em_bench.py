@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Time the abundance EM (SURVEY.md 8f rank 3) on a flattened tie-set table of nt-class size: device iteration
 (cfb_em_abundance) next to the host iteration the product uses for small tables (cfb_em_abundance_host), same table,
-and check that the two produce the same doubles and iteration counts.  usage: em_bench.py [n_species] [n_keys]"""
+and check that the two produce the same doubles and iteration counts.  usage: em_bench.py [n_species] [n_keys] [skew]
+skew (default 0): the share of keys that also name species 0, whose incidence list one device thread walks."""
 import ctypes as C
 import os
 import sys
@@ -21,6 +22,12 @@ key_off = np.concatenate([[0], np.cumsum(sz)]).astype(np.uint64)
 # reads tie within "genera" of 10 neighbouring species, as in the synthetic index
 g = rng.integers(0, n // 10, size=K)
 target = (np.repeat(g, sz) * 10 + rng.integers(0, 10, size=int(sz.sum()))).astype(np.uint32)
+skew = float(sys.argv[3]) if len(sys.argv) > 3 else 0.0
+if skew > 0:
+    extra = rng.random(K) < skew                      # these keys get species 0 as one more target, at their end
+    ends = key_off[1:].astype(np.int64)
+    target = np.insert(target, ends[extra], 0).astype(np.uint32)
+    key_off = np.concatenate([[0], np.cumsum(sz + extra)]).astype(np.uint64)
 count = rng.integers(1, 2000, size=K).astype(np.uint64)
 length = rng.integers(500000, 8000000, size=n).astype(np.uint64)
 p0 = rng.random(n); p0 /= p0.sum()
