@@ -46,7 +46,7 @@ struct IndexView {
 	const uint64_t* paths;      // n_paths * 10
 	const uint8_t*  seq_excluded;   // per-sequence flag (per ctx; may be null)
 	const uint64_t* host_taxids;    // sorted expanded host set (per ctx)
-	const uint64_t* rank16;         // device-only rank entries: 16 bytes (occ_c, 64 indicator bits) per (64 rows, base)
+	const uint64_t* rank16;         // device-only rank entries: 16 bytes (occ_c, 64 indicator bits) per (64 rows, base); format and decoders below
 	const uint64_t* ftab2;          // device-only fused ftab: (top, bot) per 10-mer, eftab already resolved
 	const uint16_t* rtab16;         // device-only resolve table: sequence id of EVERY SA row (one of rtab16/rtab32, or neither)
 	const uint32_t* rtab32;
@@ -101,6 +101,18 @@ CFB_HD uint32_t ctz32(uint32_t x) {      // x != 0
 #endif
 }
 
+// rank16 (IndexView::rank16): for every 64 rows and every base c one 16-byte entry
+//   u64 occ_c (count of c before the block, '$' excluded; bit 63 of A's entry = "block holds a genome-boundary row")  |
+//   u64 indicator bits (BWT[row] == c; the '$' row has no bit)
+// so LF(row, c) = fchr[c] + occ + popc(bits & lowmask(row & 63)).  Every kernel addresses and decodes entries through these two.
+static const uint64_t kOccMask = 0x7fffffffffffffffull;
+// index of the entry of (row, c) in 16-byte units; the four bases of a block share one 64-byte chunk
+CFB_HD uint64_t r16_entry(uint64_t row, int c) { return (row >> 6) * 4 + (uint64_t)c; }
+// LF(row, c) from the entry of (row, c)
+CFB_HD uint64_t r16_lf(const IndexView& v, uint64_t row, int c, uint64_t occ, uint64_t bits) {
+	return v.fchr[c] + (occ & kOccMask) + (uint64_t)popc64(bits & (((uint64_t)1 << (row & 63)) - 1));
+}
+
 // walk8 (k_build_walk8): per SA row r, the row eight successive mapLF1 steps reach (bits 0-39), the eight BWT bases met on the
 // way (2 bits each from bit 40, first step lowest) and the number of valid steps (bits 56-63; fewer than 8 when the walk meets
 // the '$' row).  walk8_steps = how many of the next eight read bases (`win`: 2 bits each, base p in bits 2p; N bits in `nwin`)
@@ -133,9 +145,9 @@ CFB_HD uint64_t match2(uint64_t w, int c) {
 CFB_HD int bwt_char(const IndexView& v, uint64_t row) {
 #ifdef __CUDA_ARCH__
 	if(v.rank16) {     // device replica: the indicator bits of the row's 64-row block (one 64-byte chunk); the '$' row has no bit and reads as A, as the file stores it
-		const uint64_t* e = v.rank16 + (row >> 6) * 8;
 		const uint32_t o = (uint32_t)(row & 63);
-		return (int)(((e[3] >> o) & 1ull) * 1 + ((e[5] >> o) & 1ull) * 2 + ((e[7] >> o) & 1ull) * 3);
+		auto bit = [&](int c) -> uint64_t { return (v.rank16[r16_entry(row, c) * 2 + 1] >> o) & 1ull; };
+		return (int)(bit(1) * 1 + bit(2) * 2 + bit(3) * 3);
 	}
 #endif
 	uint64_t s = row / 384; uint32_t off = (uint32_t)(row - s * 384);
@@ -148,8 +160,8 @@ CFB_HD int bwt_char(const IndexView& v, uint64_t row) {
 CFB_HD uint64_t lf_scalar(const IndexView& v, uint64_t row, int c) {
 #ifdef __CUDA_ARCH__
 	if(v.rank16) {     // device replica: one 16-byte rank16 entry (occ before the block, '$' excluded | indicator bits), same value as below
-		const uint64_t* e = v.rank16 + ((row >> 6) * 4 + (uint64_t)c) * 2;
-		return v.fchr[c] + (e[0] & 0x7fffffffffffffffull) + (uint64_t)popc64(e[1] & (((uint64_t)1 << (row & 63)) - 1));
+		const uint64_t* e = v.rank16 + r16_entry(row, c) * 2;
+		return r16_lf(v, row, c, e[0], e[1]);
 	}
 #endif
 	uint64_t s = row / 384; uint32_t off = (uint32_t)(row - s * 384);

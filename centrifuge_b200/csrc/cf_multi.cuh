@@ -216,45 +216,6 @@ __global__ void __launch_bounds__(128) k_gather_probe(const unsigned long long* 
 	}
 	if(acc == 0x123456789abcull) *sink = acc;
 }
-// The same gathers issued as bulk asynchronous copies (the TMA engine: cp.async.bulk global -> shared, completion on an
-// mbarrier) instead of LDG: every lane copies ILP 16-byte entries per round into its own shared-memory slots, the warp's
-// mbarrier collects the bytes, all lanes wait for the phase.  This is the north-star's "staged from HBM through TMA into
-// shared memory" applied to the access pattern the FM walk really has (one 16-byte entry per dependent step), so that the
-// choice between the two paths rests on a measurement of this device, not on taste.
-template <int ILP>
-__global__ void __launch_bounds__(128) k_gather_probe_bulk(const ulonglong2* __restrict__ a, uint64_t n, uint32_t iters, unsigned long long* sink, unsigned int* timeouts) {
-	__shared__ __align__(16) ulonglong2 slot[4][32 * ILP];
-	__shared__ __align__(8) unsigned long long bar[4];
-	const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-	const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	const uint32_t bar_addr = (uint32_t)__cvta_generic_to_shared(&bar[w]);
-	if(lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar_addr));
-	asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-	__syncwarp();
-	uint64_t h = gmix(tid * 0x2545F4914F6CDD1Dull + 1), acc = 0;
-	uint32_t phase = 0;
-	for(uint32_t it = 0; it < iters; it++) {
-		if(lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar_addr), "r"(32u * ILP * 16u) : "memory");
-		__syncwarp();
-		#pragma unroll
-		for(int k = 0; k < ILP; k++) {
-			h = gmix(h + k);
-			const ulonglong2* src = a + (h % n);
-			const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&slot[w][lane * ILP + k]);
-			asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], 16, [%2];" :: "r"(dst), "l"(src), "r"(bar_addr) : "memory");
-		}
-		uint32_t done = 0; const long long t0 = clock64();
-		while(!done) {
-			asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(bar_addr), "r"(phase) : "memory");
-			if(!done && clock64() - t0 > 2000000000ll) { if(lane == 0) atomicAdd(timeouts, 1u); return; }    // never hang the box on a wrong guess
-		}
-		phase ^= 1;
-		#pragma unroll
-		for(int k = 0; k < ILP; k++) { const ulonglong2 v = slot[w][lane * ILP + k]; acc += v.x ^ (v.y << 1); }
-		__syncwarp();
-	}
-	if(acc == 0x123456789abcull) *sink = acc;
-}
 // table: 0 = rank16 (16-byte entries), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it),
 // 4 = death bits, which have no table of their own (always "not built")
 extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_requests, double* g_requests_per_s, double* ms_out) {
@@ -277,19 +238,14 @@ extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_req
 	const uint32_t iters = (uint32_t)std::max<uint64_t>(1, n_requests / per_iter);
 	unsigned long long* sink = nullptr; CK(cudaMalloc((void**)&sink, 8));
 	cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-	const bool bulk = getenv("CFB_GATHER_BULK") != nullptr && W == 2;      // 16-byte entries through cp.async.bulk instead of LDG (A/B evidence only)
-	unsigned int* tmo = nullptr; CK(cudaMalloc((void**)&tmo, 4)); CK(cudaMemset(tmo, 0, 4));
 	auto launch = [&](uint32_t it) {
-		if(bulk) k_gather_probe_bulk<4><<<blocks, threads>>>(reinterpret_cast<const ulonglong2*>(base), n, it, sink, tmo);
-		else if(W == 2) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink);
+		if(W == 2) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink);
 	};
 	launch(std::max<uint32_t>(1, iters / 16)); CK(cudaDeviceSynchronize());      // warm-up
 	CK(cudaEventRecord(e0)); launch(iters); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
 	float ms = 0; CK(cudaEventElapsedTime(&ms, e0, e1));
-	unsigned int h_tmo = 0; cudaMemcpy(&h_tmo, tmo, 4, cudaMemcpyDeviceToHost);
-	cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(sink); cudaFree(tmo);
+	cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(sink);
 	CK(cudaGetLastError());
-	if(h_tmo) return fail(CFB_ECUDA, "cfb_gather_ceiling: %u warps timed out waiting for bulk copies", h_tmo);
 	*g_requests_per_s = (double)per_iter * iters / ((double)ms * 1e6);
 	if(ms_out) *ms_out = ms;
 	return CFB_OK;

@@ -31,16 +31,9 @@ struct SearchArgs {
 	unsigned int* overflow;
 	Counters* ctr;
 	const uint64_t* pk; const uint32_t* nm; uint32_t W;   // packed reads (k_pack)
-	uint32_t jump_w;                                      // widest range k_search_t advances eight bases per walk8 gather (CFB_JUMP_W; default: any width)
 	uint32_t keep_short;                                  // store every hit (min_hitlen < 22, k_search_long); else only hits of >= kLongLen bases
 };
 
-// row -> (side, offset in side).  Rows are < 2^39 for any index that fits in HBM, so row>>7 fits
-// 32 bits and the division by 3 is a single mul.hi (384 = 128 * 3).
-__device__ __forceinline__ void row_locus(uint64_t row, uint64_t& side, uint32_t& off) {
-	const uint32_t q = (uint32_t)(row >> 7) / 3u;
-	side = q; off = (uint32_t)(row - (uint64_t)q * 384u);
-}
 __device__ __forceinline__ uint64_t shl64(uint64_t v, uint32_t n) {   // PTX shl clamps n >= 64 to "all shifted out"
 	uint64_t r; asm("shl.b64 %0, %1, %2;" : "=l"(r) : "l"(v), "r"(n)); return r;
 }
@@ -141,10 +134,7 @@ __device__ __forceinline__ uint64_t even_bits(uint64_t x) {    // gather bits 0,
 }
 
 // ---------------------------------------------------------------------------------------
-// rank16: the layout both walk kernels use.  For every 64 rows and every base c one 16-byte entry
-//   u64 occ_c (count of c before the block, '$' excluded; bit 63 of A's entry = "block holds a genome-
-//   boundary row")  |  u64 indicator bits (BWT[row] == c; the '$' row has no bit)
-// so LF(row, c) = fchr[c] + occ + popc(bits & lowmask(row & 63)) costs ONE 16-byte load request.
+// rank16 (format: cf_logic.h, r16_entry / r16_lf): the layout both walk kernels use.  LF(row, c) costs ONE 16-byte load request.
 // Measured on this part (tools/gather_bench.cu): fully divergent gathers are capped at ~70 G 16-byte
 // lane requests/s independent of size (32 B: 34 G/s, 64 B: 17.6 G/s, 128 B: 8.9 G/s), so requests per
 // LF step -- not bytes -- is what bounds the walk.  The four bases of a block share one 64-byte chunk.
@@ -197,7 +187,6 @@ __host__ __device__ __forceinline__ uint32_t nh_pack(uint32_t stored, uint32_t f
 }
 __host__ __device__ __forceinline__ uint32_t nh_stored(uint32_t w) { return w & 0x7fffu; }
 __host__ __device__ __forceinline__ uint32_t nh_found(uint32_t w) { return (w >> 15) & 0x7fffu; }
-static const uint64_t kOccMask = 0x7fffffffffffffffull;
 
 // K-mer jump table: one 16-byte entry per K-mer (K >= ftabChars) that a partial search gathers in place of its first K
 // steps (hi_aligner.h:985-1008), trading HBM capacity (16 B x 4^K; 17 GB at K = 15) for random accesses.
@@ -221,14 +210,13 @@ __device__ __forceinline__ uint32_t ftabk_death(uint64_t y, uint32_t e) {
 }
 // One thread per K-mer walks the depth-3 tree of extensions; a 64-byte rank16 chunk carries the entries of all four bases of
 // a block, so every tree node costs one or two loads.
-__device__ __forceinline__ void lf4(const ulonglong2* r16, const uint64_t* fchr, uint64_t top, uint64_t bot, uint64_t t[4], uint64_t b[4]) {
-	const ulonglong2* pt = r16 + (top >> 6) * 4; const ulonglong2* pb = r16 + (bot >> 6) * 4;
-	const uint64_t mt = (1ull << (top & 63)) - 1ull, mb = (1ull << (bot & 63)) - 1ull;
+__device__ __forceinline__ void lf4(const IndexView& v, const ulonglong2* r16, uint64_t top, uint64_t bot, uint64_t t[4], uint64_t b[4]) {
+	const ulonglong2* pt = r16 + r16_entry(top, 0); const ulonglong2* pb = r16 + r16_entry(bot, 0);
 	#pragma unroll
 	for(int c = 0; c < 4; c++) {
 		const ulonglong2 et = __ldg(pt + c); const ulonglong2 eb = (pb == pt) ? et : __ldg(pb + c);
-		t[c] = fchr[c] + (et.x & 0x7fffffffffffffffull) + (uint64_t)__popcll(et.y & mt);
-		b[c] = fchr[c] + (eb.x & 0x7fffffffffffffffull) + (uint64_t)__popcll(eb.y & mb);
+		t[c] = r16_lf(v, top, c, et.x, et.y);
+		b[c] = r16_lf(v, bot, c, eb.x, eb.y);
 	}
 }
 __global__ void __launch_bounds__(128) k_build_ftabk(IndexView v, int K, uint64_t n, bool death, ulonglong2* out) {
@@ -240,22 +228,22 @@ __global__ void __launch_bounds__(128) k_build_ftabk(IndexView v, int K, uint64_
 	uint64_t top = v.ftab2[f10 * 2], bot = v.ftab2[f10 * 2 + 1];
 	for(int j = fc; j < K && bot > top; j++) {
 		const int c = (int)((fk >> (2 * j)) & 3);
-		const ulonglong2 tq = __ldg(r16 + (top >> 6) * 4 + c), bq = __ldg(r16 + (bot >> 6) * 4 + c);
-		top = v.fchr[c] + (tq.x & kOccMask) + (uint64_t)__popcll(tq.y & ((1ull << (top & 63)) - 1ull));
-		bot = v.fchr[c] + (bq.x & kOccMask) + (uint64_t)__popcll(bq.y & ((1ull << (bot & 63)) - 1ull));
+		const ulonglong2 tq = __ldg(r16 + r16_entry(top, c)), bq = __ldg(r16 + r16_entry(bot, c));
+		top = r16_lf(v, top, c, tq.x, tq.y);
+		bot = r16_lf(v, bot, c, bq.x, bq.y);
 	}
 	if(bot <= top) { out[fk] = make_ulonglong2(0ull, ~0ull); return; }
 	uint64_t y = ~0ull;
 	if(death) {
 		// true death depth of every extension (0 = the (K+3)-mer occurs), then the bitmap, kept only if it decodes to them all
 		uint8_t dv[64];
-		uint64_t t1[4], b1[4]; lf4(r16, v.fchr, top, bot, t1, b1);
+		uint64_t t1[4], b1[4]; lf4(v, r16, top, bot, t1, b1);
 		for(int c0 = 0; c0 < 4; c0++) {
 			if(b1[c0] <= t1[c0]) { for(int r = 0; r < 16; r++) dv[c0 | (r << 2)] = 1; continue; }
-			uint64_t t2[4], b2[4]; lf4(r16, v.fchr, t1[c0], b1[c0], t2, b2);
+			uint64_t t2[4], b2[4]; lf4(v, r16, t1[c0], b1[c0], t2, b2);
 			for(int c1 = 0; c1 < 4; c1++) {
 				if(b2[c1] <= t2[c1]) { for(int c2 = 0; c2 < 4; c2++) dv[c0 | (c1 << 2) | (c2 << 4)] = 2; continue; }
-				uint64_t t3[4], b3[4]; lf4(r16, v.fchr, t2[c1], b2[c1], t3, b3);
+				uint64_t t3[4], b3[4]; lf4(v, r16, t2[c1], b2[c1], t3, b3);
 				for(int c2 = 0; c2 < 4; c2++) dv[c0 | (c1 << 2) | (c2 << 4)] = b3[c2] <= t3[c2] ? 3 : 0;
 			}
 		}
@@ -306,10 +294,10 @@ template <int RW> struct ReadRegs {
 	}
 };
 
-// COUNT: 0 = product; 1 = the reference's operation counters (SURVEY 8d: jump tables off, so that the operation sequence is the
-// reference's); 2 = the product's own load requests with every table live (what the roofline of *this* kernel is made of)
-template <int COUNT, int RW>
-__global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1) k_search_t(const SearchArgs a) {
+// REQS: count the product's own load requests with every table live (what the roofline of *this* kernel is made of).  The
+// reference's operation counters come from search_strand_scalar (k_search_long<true>).
+template <bool REQS, int RW>
+__global__ void __launch_bounds__(kSearchThreads, !REQS && RW <= 5 ? 8 : 1) k_search_t(const SearchArgs a) {
 	// RW = 4: 56 registers, 8 CTAs per SM; RW = 5 keeps 8 CTAs through the launch bounds (62 registers, no spills).  Forcing 9
 	// for RW = 4 (then at 58 registers; 56 with the bound, no spills) took the search kernel from 28.0 to 27.4 ms per 10 M reads on
 	// one H100 80GB HBM3 at 400 W, but reads/s moved by about one run-to-run spread (256.4 vs 259.7 M, three runs each), so it is
@@ -317,9 +305,9 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(a.v.rank16);
 	const ulonglong2* ftab2 = reinterpret_cast<const ulonglong2*>(a.v.ftab2);
 	const ulonglong2* ftabk = reinterpret_cast<const ulonglong2*>(a.v.ftabk);
-	const uint32_t fk = (COUNT == 1 || !a.v.ftabk) ? 0u : (uint32_t)a.v.ftabk_chars;   // counters follow the reference's op sequence
+	const uint32_t fk = a.v.ftabk ? (uint32_t)a.v.ftabk_chars : 0u;
 	const uint32_t fc = (uint32_t)a.v.ftab_chars;
-	const unsigned long long* w8 = COUNT == 1 ? nullptr : reinterpret_cast<const unsigned long long*>(a.v.walk8);
+	const unsigned long long* w8 = reinterpret_cast<const unsigned long long*>(a.v.walk8);
 	// death bitmap of the K-mer table (fd = K + 3): only while every hit it can end (at most fd - 1 bases) stays below
 	// min_hitlen, i.e. is never resolved
 	const uint32_t fd = (fk == 0 || a.p.min_hitlen < (uint32_t)a.v.ftabd_chars) ? 0u : (uint32_t)a.v.ftabd_chars;
@@ -328,7 +316,6 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 	uint32_t rlen = 0, tid = 0, cur = 0, dep = 0, offset = 0, nh = 0, nt = 0, slow_until = 0, fail_at = 0xffffffffu;
 	bool nolong = true;      // no hit of this strand reaches min_hitlen (kListNoLong tells the per-unit kernels)
 	int mode = M_NEED;
-	unsigned long long c_ps = 0, c_ft = 0, c_sides = 0, c_lf = 0;
 	unsigned long long q_r16 = 0, q_f2 = 0, q_fk = 0, q_w8 = 0;
 	unsigned long long q_w1 = 0, q_w24 = 0, q_w5 = 0, j_row = 0, j_row_ok = 0, j_rng = 0, j_rng_ok = 0, j_w5_ok = 0;
 	WarpPool pool; pool.base = pool.end = 0;
@@ -353,7 +340,6 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 	// partialSearch prologue (hi_aligner.h:939-982) at `cur`: ends in M_FTAB (fi set) or M_NEED
 	auto start_search = [&]() {
 		for(;;) {
-			if(COUNT == 1) c_ps++;
 			offset = cur;
 			if(rlen - cur < fc) { emit(kOff, kOff, offset, rlen - offset); a.nhits[tid] = nh_pack(nh, nt, nolong); mode = M_NEED; return; }
 			uint64_t win; uint32_t nwin; rd.window(cur, win, nwin);
@@ -415,25 +401,25 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 		const bool lf = mode == M_LF;
 		bool range = false, jump = false, known_fail = false;
 		const void* p0 = nullptr; const void* p1 = nullptr; uint32_t sub = 0;
-		if(mode == M_FTAB) { p0 = ftab2 + fi; if(COUNT == 2) q_f2++; }                                // (top, bot) of the 10-mer
-		else if(mode == M_FTABK) { p0 = ftabk + (fi & ((1ull << (2 * fk)) - 1ull)); if(COUNT == 2) q_fk++; }   // range + death bitmap of the K-mer
+		if(mode == M_FTAB) { p0 = ftab2 + fi; if(REQS) q_f2++; }                                // (top, bot) of the 10-mer
+		else if(mode == M_FTABK) { p0 = ftabk + (fi & ((1ull << (2 * fk)) - 1ull)); if(REQS) q_fk++; }   // range + death bitmap of the K-mer
 		else if(lf) {
 			c = rd.base(dep);
 			if(c <= 3) {
 				range = (bot - top) != 1;
 				const uint64_t width = bot - top;
 				if(dep == fail_at && !range) known_fail = true;      // the walk8 entry already said that this step of the single row fails: no request
-				else if(w8 && width <= (uint64_t)a.jump_w && dep >= slow_until && rlen - dep >= 8 && bot <= a.v.walk8_rows) {
+				else if(w8 && dep >= slow_until && rlen - dep >= 8 && bot <= a.v.walk8_rows) {
 					// Eight steps in one gather: the read's next eight bases are the ones stored for the range's first AND last
 					// row.  Then the range after them is exactly [W8(top), W8(bot - 1) + 1), whatever the rows in between do
 					// (cf_logic.h, walk8_steps).  One 16-byte piece serves both ends when they share it.
 					jump = true; p0 = w8 + (top & ~1ull); sub = (uint32_t)(top & 1);
 					if(range) { const uint64_t last = bot - 1; sub |= (uint32_t)(last & 1) << 1; if((last & ~1ull) != (top & ~1ull)) p1 = w8 + (last & ~1ull); }
-					if(COUNT == 2) { q_w8 += p1 ? 2 : 1; if(range) j_rng++; else j_row++; }
+					if(REQS) { q_w8 += p1 ? 2 : 1; if(range) j_rng++; else j_row++; }
 				} else {
-					p0 = r16 + (top >> 6) * 4 + c;                          // (occ, bits): one request per rank query
-					if(range && (bot >> 6) != (top >> 6)) p1 = r16 + (bot >> 6) * 4 + c;
-					if(COUNT == 2) { const uint32_t n = p1 ? 2 : 1; q_r16 += n; if(width == 1) q_w1 += n; else if(width <= 4) q_w24 += n; else q_w5 += n; }
+					p0 = r16 + r16_entry(top, c);                           // (occ, bits): one request per rank query
+					if(range && (bot >> 6) != (top >> 6)) p1 = r16 + r16_entry(bot, c);
+					if(REQS) { const uint32_t n = p1 ? 2 : 1; q_r16 += n; if(width == 1) q_w1 += n; else if(width <= 4) q_w24 += n; else q_w5 += n; }
 				}
 			}
 		}
@@ -457,7 +443,6 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 				if(dep < rlen) mode = M_LF; else hit_and_restart();
 			} else { fi &= (1ull << (2 * fc)) - 1ull; mode = M_FTAB; }   // died between base fc and K, or too wide: replay from the 10-mer
 		} else if(mode == M_FTAB) {
-			if(COUNT == 1) c_ft++;
 			top = e.x; bot = e.y;
 			dep = cur + fc;
 			if(bot <= top) {                              // hi_aligner.h:971-982
@@ -473,7 +458,7 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 			const uint64_t wl = range ? ((sub & 2u) ? bq.y : bq.x) : w;      // entry of the last row
 			const uint32_t st = walk8_steps(w, win, nwin), sb = range ? walk8_steps(wl, win, nwin) : st;
 			if((st & sb) == 8u) {                                            // both end rows follow all eight bases
-				if(COUNT == 2) { if(range) j_rng_ok++; else j_row_ok++; if(bot - top >= 5) j_w5_ok++; }
+				if(REQS) { if(range) j_rng_ok++; else j_row_ok++; if(bot - top >= 5) j_w5_ok++; }
 				top = w & kWalkRowMask; bot = (wl & kWalkRowMask) + 1; dep += 8;
 				if(dep >= rlen) hit_and_restart();
 			} else {      // an end row leaves within the next eight steps: take them one by one until both failing ends have left
@@ -484,29 +469,19 @@ __global__ void __launch_bounds__(kSearchThreads, COUNT == 0 && RW <= 5 ? 8 : 1)
 			bool fail = c > 3 || known_fail;
 			uint64_t t = 0, b = 0;
 			if(!fail) {
-				const uint32_t oT = (uint32_t)(top & 63), oB = (uint32_t)(bot & 63);
-				t = a.v.fchr[c] + (tq.x & kOccMask) + (uint64_t)__popcll(tq.y & ((1ull << oT) - 1ull));
-				if(range) b = a.v.fchr[c] + (bq.x & kOccMask) + (uint64_t)__popcll(bq.y & ((1ull << oB) - 1ull));
+				t = r16_lf(a.v, top, c, tq.x, tq.y);
+				if(range) b = r16_lf(a.v, bot, c, bq.x, bq.y);
 				else {                                    // mapLF1 bt2_idx.h:2910-2933: BWT[top] must be c ('$' has no bit)
-					if(!((tq.y >> oT) & 1ull)) fail = true;
+					if(!((tq.y >> (top & 63)) & 1ull)) fail = true;
 					b = t + 1;
 				}
 				if(b <= t) fail = true;
-				if(COUNT == 1) {   // counters keep the reference's side geometry (384 rows per 128-byte side)
-					uint64_t sT; uint32_t offT; row_locus(top, sT, offT);
-					const bool same_side = !range || (bot - top) < (uint64_t)(384 - offT);
-					c_lf += range ? 2 : 1; c_sides += same_side ? 1 : 2;
-				}
 			}
 			if(fail) hit_and_restart();
 			else { top = t; bot = b; dep++; if(dep >= rlen) hit_and_restart(); }
 		}
 	}
-	if(COUNT == 1 && a.ctr) {
-		atomicAdd(&a.ctr->partial_searches, c_ps); atomicAdd(&a.ctr->ftab_probes, c_ft);
-		atomicAdd(&a.ctr->sides_search, c_sides); atomicAdd(&a.ctr->lf_steps, c_lf);
-	}
-	if(COUNT == 2 && a.ctr) {
+	if(REQS && a.ctr) {
 		atomicAdd(&a.ctr->req_rank16, q_r16); atomicAdd(&a.ctr->req_ftab2, q_f2); atomicAdd(&a.ctr->req_ftabk, q_fk); atomicAdd(&a.ctr->req_walk8, q_w8);
 		atomicAdd(&a.ctr->r16_w1, q_w1); atomicAdd(&a.ctr->r16_w2_4, q_w24); atomicAdd(&a.ctr->r16_w5, q_w5);
 		atomicAdd(&a.ctr->w8_try_row, j_row); atomicAdd(&a.ctr->w8_ok_row, j_row_ok); atomicAdd(&a.ctr->w8_try_range, j_rng); atomicAdd(&a.ctr->w8_ok_range, j_rng_ok); atomicAdd(&a.ctr->w8_ok_w5, j_w5_ok);
@@ -572,14 +547,13 @@ __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const
 							slow_until = dep + walk8_retry(st, sb);
 						}
 						if(bot - top == 1) {
-							const ulonglong2 e = __ldg(r16 + (top >> 6) * 4 + c);
+							const ulonglong2 e = __ldg(r16 + r16_entry(top, c));
 							if(!((e.y >> (top & 63)) & 1ull)) break;                      // mapLF1: BWT[top] must be c ('$' has no bit)
-							top = v.fchr[c] + (e.x & kOccMask) + (uint64_t)__popcll(e.y & ((1ull << (top & 63)) - 1ull)); bot = top + 1; dep++;
+							top = r16_lf(v, top, c, e.x, e.y); bot = top + 1; dep++;
 						} else {
-							const ulonglong2 et = __ldg(r16 + (top >> 6) * 4 + c);
-							const ulonglong2 eb = (bot >> 6) == (top >> 6) ? et : __ldg(r16 + (bot >> 6) * 4 + c);
-							const uint64_t t = v.fchr[c] + (et.x & kOccMask) + (uint64_t)__popcll(et.y & ((1ull << (top & 63)) - 1ull));
-							const uint64_t b = v.fchr[c] + (eb.x & kOccMask) + (uint64_t)__popcll(eb.y & ((1ull << (bot & 63)) - 1ull));
+							const ulonglong2 et = __ldg(r16 + r16_entry(top, c));
+							const ulonglong2 eb = (bot >> 6) == (top >> 6) ? et : __ldg(r16 + r16_entry(bot, c));
+							const uint64_t t = r16_lf(v, top, c, et.x, et.y), b = r16_lf(v, bot, c, eb.x, eb.y);
 							if(b <= t) break;
 							top = t; bot = b; dep++;
 						}
@@ -600,10 +574,10 @@ __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const
 
 // k_search_long: batches with a read longer than k_search_t's widest register window (kWindowLen bases).  One thread per
 // (unit, mate, strand) task runs the strand's whole search from the byte form of the read and stores every hit, so k_prep
-// never regenerates these lists.  COUNT == 1 runs search_strand_scalar, which counts the reference's operations; COUNT == 2
-// counts no load requests for these reads.
+// never regenerates these lists.  SCALAR runs search_strand_scalar, one LF step at a time with the jump tables off, for every read
+// length: the pass that counts the reference's operations (SURVEY 8d).  The table walk counts no load requests for these reads.
 static const uint32_t kWindowLen = 320;      // 10 register words of 32 bases
-template <int COUNT>
+template <bool SCALAR>
 __global__ void __launch_bounds__(kSearchThreads) k_search_long(const SearchArgs a) {
 	const uint32_t per = 2u * (uint32_t)a.b.n_mates;
 	Counters local; memset(&local, 0, sizeof local);
@@ -615,24 +589,27 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_long(const SearchArgs
 		if(!((fl >> mate) & 1) || len == 0) { a.nhits[tid] = 0; continue; }
 		const uint8_t* fw = a.b.bases + a.b.off[mate][unit];
 		HitRec* hits = a.hits + (size_t)tid * a.cap;
-		const uint32_t n = COUNT == 1 ? search_strand_scalar(a.v, a.p, fw, len, strand, hits, a.cap, &local)
-		                              : search_strand_dev(a.v, a.p, fw, len, strand, hits, a.cap);
+		const uint32_t n = SCALAR ? search_strand_scalar(a.v, a.p, fw, len, strand, hits, a.cap, &local)
+		                          : search_strand_dev(a.v, a.p, fw, len, strand, hits, a.cap);
 		if(n > a.cap) atomicExch(a.overflow, 1u);      // the host grows the lists and re-runs the batch
 		a.nhits[tid] = nh_pack(min(n, a.cap), n, false);
 	}
-	if(COUNT == 1 && a.ctr) {
+	if(SCALAR && a.ctr) {
 		atomicAdd(&a.ctr->partial_searches, local.partial_searches); atomicAdd(&a.ctr->ftab_probes, local.ftab_probes);
 		atomicAdd(&a.ctr->sides_search, local.sides_search); atomicAdd(&a.ctr->lf_steps, local.lf_steps);
 	}
 }
 
 typedef void (*SearchKernel)(const SearchArgs);
-// the thread-per-walk kernel whose register window holds the batch's longest read
+// count 1: the scalar search, which counts the reference's operations; otherwise the thread-per-walk kernel whose register
+// window holds the batch's longest read (count 2: its request-counting instantiation)
 static SearchKernel search_kernel(uint32_t maxlen, int count) {
-	if(maxlen > kWindowLen) return count == 2 ? k_search_long<2> : (count ? k_search_long<1> : k_search_long<0>);
-	if(maxlen > 160) return count == 2 ? k_search_t<2, 10> : (count ? k_search_t<1, 10> : k_search_t<0, 10>);
-	if(maxlen > 128) return count == 2 ? k_search_t<2, 5> : (count ? k_search_t<1, 5> : k_search_t<0, 5>);      // 2 x 150 bp runs
-	return count == 2 ? k_search_t<2, 4> : (count ? k_search_t<1, 4> : k_search_t<0, 4>);
+	if(count == 1) return k_search_long<true>;
+	if(maxlen > kWindowLen) return k_search_long<false>;
+	const bool reqs = count == 2;
+	if(maxlen > 160) return reqs ? k_search_t<true, 10> : k_search_t<false, 10>;
+	if(maxlen > 128) return reqs ? k_search_t<true, 5> : k_search_t<false, 5>;      // 2 x 150 bp runs
+	return reqs ? k_search_t<true, 4> : k_search_t<false, 4>;
 }
 
 // found[r][st] receives the number of hits the search found for the list (0 for a regenerated list); tpos[r] the index of
@@ -851,6 +828,17 @@ struct ResolveArgs {
 	IndexView v; const uint64_t* rows; uint32_t* ids; uint16_t* ids16; const uint64_t* total; uint64_t rows_cap;
 	unsigned long long* task_ctr; uint32_t chunk; Counters* ctr;
 };
+// One LF step of a 4-lane group (k_resolve_c, k_build_walk8): lane j holds base j's rank16 entry `e` of row's block; the lane
+// whose indicator bit is set at the row owns BWT[row] and its LF value is the next row.  Returns that base, or -1 where no lane
+// owns the row (the '$' row; `next` is then meaningless).
+__device__ __forceinline__ int group_lf(const IndexView& v, uint64_t row, const ulonglong2 e, uint64_t& next) {
+	const unsigned gl = threadIdx.x & 3, gbase = threadIdx.x & 28, gmask = 0xFu << gbase;
+	const uint64_t mine = r16_lf(v, row, (int)gl, e.x, e.y);
+	const int src = __ffs((__ballot_sync(gmask, (e.y >> (row & 63)) & 1ull) >> gbase) & 0xFu) - 1;
+	next = __shfl_sync(gmask, mine, gbase + (src < 0 ? 0 : src));
+	return src;
+}
+
 // ---------------------------------------------------------------------------------------
 // k_resolve_c: 4 lanes per SA row over rank16.  Lane j fetches the entry of base j, so the 64-byte
 // chunk of a block arrives with ONE load request per walk step; the lane whose indicator bit is set
@@ -891,11 +879,10 @@ __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs 
 		}
 		if(!__any_sync(0xffffffffu, mode != R_DONE)) break;
 		ulonglong2 e = make_ulonglong2(0, 0); uint32_t samp = 0;
-		if(mode == R_WALK) e = __ldg(r16 + (row >> 6) * 4 + gl);
+		if(mode == R_WALK) e = __ldg(r16 + r16_entry(row, (int)gl));
 		else if(mode == R_SAMPLE && gl == 0) samp = a.v.sample32 ? __ldg(a.v.sample32 + (row >> a.v.off_rate)) : (uint32_t)__ldg(a.v.sample16 + (row >> a.v.off_rate));
 		if(mode == R_SAMPLE) { if(gl == 0) put(samp); mode = R_NEED; }
 		else if(mode == R_WALK) {
-			const uint32_t off = (uint32_t)(row & 63);
 			const unsigned flagged = __shfl_sync(gmask, (unsigned)(e.x >> 63), gbase);     // A's entry carries the boundary flag
 			bool found = false;
 			if(flagged && a.v.last_boundary > 0 && row <= a.v.last_boundary) {
@@ -905,10 +892,7 @@ __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs 
 			}
 			if(found) mode = R_NEED;
 			else {
-				const uint64_t mine = a.v.fchr[gl] + (e.x & kOccMask) + (uint64_t)__popcll(e.y & ((1ull << off) - 1ull));
-				const unsigned who = (__ballot_sync(gmask, (e.y >> off) & 1ull) >> gbase) & 0xFu;      // exactly one base owns the row
-				const int src = __ffs(who) - 1;
-				row = __shfl_sync(gmask, mine, gbase + (src < 0 ? 0 : src));
+				group_lf(a.v, row, e, row);      // exactly one base owns the row: settle() took the '$' row
 				if(COUNT && gl == 0) c_walk++;
 				mode = settle(row);
 			}
@@ -923,7 +907,7 @@ __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs 
 // bases equal the stored ones, eight dependent rank gathers collapse into this one 8-byte gather.
 // 4 lanes per row (lane j fetches base j's rank16 entry: the 64-byte chunk is one request).
 __global__ void __launch_bounds__(kSearchThreads) k_build_walk8(IndexView v, uint64_t nrows, uint64_t* out) {
-	const unsigned lane = threadIdx.x & 31, gl = lane & 3, gbase = lane & 28, gmask = 0xFu << gbase;
+	const unsigned gl = threadIdx.x & 3;
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(v.rank16);
 	const uint64_t ngroups = (uint64_t)gridDim.x * (kSearchThreads / 4);
 	const uint64_t per = (nrows + ngroups - 1) / ngroups;
@@ -933,14 +917,11 @@ __global__ void __launch_bounds__(kSearchThreads) k_build_walk8(IndexView v, uin
 		uint64_t row = idx, chars = 0; uint32_t nv = 0;
 		for(; nv < 8; nv++) {
 			if(row == v.zoff) break;
-			const ulonglong2 e = __ldg(r16 + (row >> 6) * 4 + gl);
-			const uint32_t off = (uint32_t)(row & 63);
-			const uint64_t mine = v.fchr[gl] + (e.x & kOccMask) + (uint64_t)__popcll(e.y & ((1ull << off) - 1ull));
-			const unsigned who = (__ballot_sync(gmask, (e.y >> off) & 1ull) >> gbase) & 0xFu;
-			const int src = __ffs(who) - 1;
+			uint64_t next;
+			const int src = group_lf(v, row, __ldg(r16 + r16_entry(row, (int)gl)), next);
 			if(src < 0) break;
 			chars |= (uint64_t)src << (2 * nv);
-			row = __shfl_sync(gmask, mine, gbase + src);
+			row = next;
 		}
 		if(gl == 0) out[idx] = (row & kWalkRowMask) | (chars << 40) | ((uint64_t)nv << 56);
 	}
@@ -1310,7 +1291,7 @@ struct cfb_ctx {
 	uint64_t rows_cap0 = 0;       // CFB_ROWS_CAP: initial row-buffer capacity (tests force the grow-and-re-run path with it)
 	TextCtx* text = nullptr;
 	CountsCtx cnt; bool fold_records = false;
-	uint32_t jump_w = 0xffffffffu; bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
+	bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
 	uint64_t regen_lists = 0, regen_tasks = 0;   // lists regenerated / strand lists searched so far (CFB_REGEN_STATS=1 prints them when the context goes)
 	uint64_t regen_slots0 = 0;    // CFB_REGEN_SLOTS: initial capacity of the list-regeneration buffer (tests force the grow-and-re-run path with it)
 	void* comm = nullptr; int comm_rank = 0, comm_size = 1; cudaStream_t comm_st = nullptr;      // NCCL communicator (cf_multi.cuh)
@@ -1383,28 +1364,15 @@ extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx*
 		CKC(c->slots[i].scal.ensure(8)); CKC(c->slots[i].h_scal.ensure(8));
 	}
 	CKC(cudaMalloc((void**)&c->d_ctr, sizeof(Counters))); CKC(cudaMemset(c->d_ctr, 0, sizeof(Counters)));
-	{   // random 32-byte sector gathers: do not let L2 over-fetch neighbouring sectors from HBM
-		const char* e = getenv("CFB_L2_FETCH"); const size_t g = e ? (size_t)atoi(e) : 32;
-		if(g == 32 || g == 64 || g == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, g);
-		const char* pe = getenv("CFB_L2_PERSIST");
-		if(pe && pe[0] == '1') {   // keep the 8.4 MB ftab resident in L2 (hit by every partial search)
-			cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 16u << 20);
-			for(int i = 0; i < kSlots; i++) {
-				cudaStreamAttrValue av; memset(&av, 0, sizeof av);
-				av.accessPolicyWindow.base_ptr = (void*)c->view.ftab; av.accessPolicyWindow.num_bytes = h.ftab.size() * 8;
-				av.accessPolicyWindow.hitRatio = 1.0f; av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting; av.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-				cudaStreamSetAttribute(c->slots[i].st, cudaStreamAttributeAccessPolicyWindow, &av);
-			}
-		}
-		cudaGetLastError();
-	}
+	// random 32-byte sector gathers: do not let L2 over-fetch neighbouring sectors from HBM
+	cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
+	cudaGetLastError();
 	int occ = 0;
 	CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_resolve_c<false, false>, kSearchThreads, 0));
 	c->resolve_blocks = ix->sm_count * std::max(occ, 1);
 	{ const char* rc0 = getenv("CFB_ROWS_CAP"); if(rc0) c->rows_cap0 = strtoull(rc0, NULL, 10); }
 	{ const char* ks = getenv("CFB_KEEP_SHORT"); c->keep_short = ks && ks[0] == '1'; }
 	{ const char* rs = getenv("CFB_REGEN_SLOTS"); if(rs) c->regen_slots0 = strtoull(rs, NULL, 10); }
-	{ const char* jw = getenv("CFB_JUMP_W"); c->jump_w = jw && atoi(jw) > 0 ? (uint32_t)atoi(jw) : 0xffffffffu; }      // A/B cap on the range width of a walk8 jump (unset or 0: any width)
 	const char* cnt = getenv("CFB_COUNT");
 	c->count = cnt ? (cnt[0] == '1' ? 1 : (cnt[0] == '2' ? 2 : 0)) : 0;
 	#undef CKC
@@ -1635,8 +1603,10 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	const uint64_t scan_blocks = (n + kScanBlock * kScanPer - 1) / (kScanBlock * kScanPer);
 	if(n == 0) return CFB_OK;
 	// which search kernel runs decides what it stores: k_search_t keeps only hits of >= kLongLen bases when min_hitlen allows
-	// it (see kListRegen), k_search_long and small min_hitlen keep every hit
-	const bool keep_short = s.maxlen > kWindowLen || c->prm.min_hitlen < kLongLen || c->keep_short;
+	// it (see kListRegen); k_search_long -- for long reads, and the scalar search of a CFB_COUNT=1 pass at any read length --
+	// and small min_hitlen keep every hit
+	const SearchKernel search = search_kernel(s.maxlen, c->count);
+	const bool keep_short = search == k_search_long<true> || search == k_search_long<false> || c->prm.min_hitlen < kLongLen || c->keep_short;
 	if(stage == 0) {
 		if(s.cap == 0) {
 			s.full_cap = s.maxlen / 4 + 8;      // >= #Ns allowed by the N filter (0.15 len) + len/10 + slack
@@ -1667,11 +1637,10 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	if(stage == 0) {
 		SearchArgs sa; sa.v = c->view; sa.p = c->prm; sa.b = s.bv; sa.hits = s.hits.p; sa.nhits = s.nhits.p; sa.cap = s.cap;
 		const uint32_t W = (s.maxlen + 31) / 32 + 1;
-		sa.pk = s.pk.p; sa.nm = s.nm.p; sa.W = W; sa.jump_w = c->jump_w; sa.keep_short = keep_short ? 1u : 0u;
+		sa.pk = s.pk.p; sa.nm = s.nm.p; sa.W = W; sa.keep_short = keep_short ? 1u : 0u;
 		{ PackArgs pa; pa.b = s.bv; pa.pk = s.pk.p; pa.nm = s.nm.p; pa.W = W;
 		  k_pack<<<(unsigned)((ntasks * W + 127) / 128), 128, 0, s.st>>>(pa); c->launches++; }
 		sa.task_ctr64 = s.scal.p + 0; sa.ntasks = (uint32_t)ntasks; sa.overflow = (unsigned int*)(s.scal.p + 2); sa.ctr = ctr;
-		const SearchKernel search = search_kernel(s.maxlen, c->count);
 		int occ = 1;
 		CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, search, kSearchThreads, 0));
 		const uint64_t resident = (uint64_t)c->ix->sm_count * (uint64_t)std::max(occ, 1);

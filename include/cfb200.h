@@ -266,7 +266,8 @@ int cfb_ctx_requests(cfb_ctx*, uint64_t out[5]);
 int cfb_ctx_request_breakdown(cfb_ctx*, uint64_t out[8]);
 int cfb_gather_ceiling(const cfb_index*, int table, uint64_t n_requests, double* g_requests_per_s, double* ms);
 
-/* Operation counters of the last batch on this ctx (same definition as SURVEY.md 8d):
+/* Operation counters of the last batch on this ctx when it was created with CFB_COUNT=1, which searches with the scalar,
+ * table-free restatement of the reference's walk (same definition as SURVEY.md 8d):
  * {units, partial_searches, ftab_probes, sides_search, walk_steps, rows_resolved, lf_steps_total, ext_searches} */
 int cfb_ctx_counters(cfb_ctx*, uint64_t out[8]);
 int cfb_ctx_kernel_launches(const cfb_ctx*, uint64_t* n);

@@ -55,7 +55,8 @@ def test_long_reads_match_oracle(opt):
 
 
 def test_long_read_counters_match_host_logic(monkeypatch):
-    """k_search_long's counting instantiation counts the reference's operations, as k_search_t's does."""
+    """CFB_COUNT=1 on reads over 320 bases: the scalar search (search_strand_scalar, the host logic's own search) counts the
+    reference's operations on the device, as it does for reads of every length."""
     monkeypatch.setenv("CFB_COUNT", "1")
     from centrifuge_b200 import capi as m
     base, seqs = syn_a()

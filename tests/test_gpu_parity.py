@@ -93,10 +93,8 @@ LAYOUT_VARIANTS = {
     "no_ftabd": {"CFB_FTABD": "0"},
     "ftabd_over_ftabk12": {"CFB_FTABK": "12"},
     "half_walk8": {"CFB_WALK8_ROWS": "300000"},
-    "range_jump_w1": {"CFB_JUMP_W": "1"},
     "every_hit_stored": {"CFB_KEEP_SHORT": "1"},
     "tiny_regeneration_buffer": {"CFB_REGEN_SLOTS": "8"},      # both-strand reads overflow the side buffer: grow and re-run
-    "range_jump_w8_half_walk8": {"CFB_JUMP_W": "8", "CFB_WALK8_ROWS": "300000"},
     "no_tables": {"CFB_WALK8": "0", "CFB_RESOLVE_TABLE": "0", "CFB_FTABK": "10", "CFB_FTABD": "0"},
     "ftabk11": {"CFB_FTABK": "11"},
     "ftabk12_walk_resolve": {"CFB_FTABK": "12", "CFB_RESOLVE_TABLE": "0"},

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Random-gather ceilings of this device over the bench index replica's own arrays: LDG (what the walk kernel uses)
-next to cp.async.bulk / TMA (what the north-star design sketched), per table."""
+"""Random-gather ceilings of this device over the bench index replica's own arrays, per table: independent 16- or 8-byte LDG
+requests, the load the walk kernels use."""
 import os
 import sys
 
@@ -23,11 +23,4 @@ for t in (0, 1, 2, 3):
         print("LDG   %-45s %7.2f G requests/s  (%.1f ms)" % (names[t], g, ms))
     except capi.CfbError as e:
         print("LDG   %-45s not built (%s)" % (names[t], e))
-os.environ["CFB_GATHER_BULK"] = "1"
-for t in (0, 1):
-    try:
-        g, ms = capi.gather_ceiling(ix, t, 1 << 29)
-        print("bulk  %-45s %7.2f G requests/s  (%.1f ms)   cp.async.bulk 16 B -> shared memory, mbarrier completion, 4 copies per lane per round" % (names[t], g, ms))
-    except capi.CfbError as e:
-        print("bulk  %-45s failed: %s" % (names[t], e))
 ix.close()
