@@ -331,6 +331,13 @@ class Context:
         names = ["rank16_w1", "rank16_w2_4", "rank16_w5", "walk8_try_row", "walk8_ok_row", "walk8_try_range", "walk8_ok_range", "walk8_ok_w5"]
         return dict(zip(names, [int(x) for x in out]))
 
+    def search_iter_stats(self):
+        """how k_search_t's loop spent its trips in the last batch (CFB_COUNT=2); clocks are SM cycles summed over one lane per warp"""
+        out = (C.c_uint64 * 8)()
+        _ck(lib().cfb_ctx_search_iter_stats(self.h, out))
+        names = ["warp_iters", "lane_requests", "consumer_paths", "restart_paths", "task_iters", "clk_head", "clk_wait", "clk_tail"]
+        return dict(zip(names, [int(x) for x in out]))
+
     def counters(self):
         out = (C.c_uint64 * 8)()
         _ck(lib().cfb_ctx_counters(self.h, out))
@@ -368,6 +375,13 @@ def gather_ceiling(index, table, n_requests=1 << 30):
     """G requests/s of independent random gathers over one of the replica's arrays (0 rank16, 1 K-mer table, 2 walk8, 3 resolve table)"""
     g, ms = C.c_double(), C.c_double()
     _ck(lib().cfb_gather_ceiling(index.h, C.c_int(table), C.c_uint64(n_requests), C.byref(g), C.byref(ms)))
+    return float(g.value), float(ms.value)
+
+
+def gather_rate(index, table, n_requests, ctas_per_sm, ilp):
+    """the gather_ceiling probe with ctas_per_sm x 128 x ilp requests in flight per SM (the ceiling itself is 16, 4)"""
+    g, ms = C.c_double(), C.c_double()
+    _ck(lib().cfb_gather_rate(index.h, C.c_int(table), C.c_uint64(n_requests), C.c_int(ctas_per_sm), C.c_int(ilp), C.byref(g), C.byref(ms)))
     return float(g.value), float(ms.value)
 
 

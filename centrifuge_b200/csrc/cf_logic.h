@@ -84,6 +84,11 @@ struct Counters {   // algorithmic-operation counters (SURVEY.md section 8d defi
 	// where the requests of count mode 2 go: rank16 requests made while the range has width 1, 2-4 and >= 5 (they sum to
 	// req_rank16), and walk8 jumps tried and taken from a single row and from a range (w8_ok_w5: taken from width >= 5)
 	unsigned long long r16_w1, r16_w2_4, r16_w5, w8_try_row, w8_ok_row, w8_try_range, w8_ok_range, w8_ok_w5;
+	// how k_search_t's loop spends a trip (count mode 2): warp-iterations, lane-iterations that issued a table request,
+	// distinct consumer branches and distinct restart blocks (hit store, hand-out, search start) with at least one lane,
+	// summed over warp-iterations, warp-iterations in which a lane received a task, and SM clocks summed by lane 0 over
+	// loop top -> fetch issue, fetch issue -> loaded data usable, loaded data usable -> end of the trip
+	unsigned long long it_warp, it_lane_req, it_consumers, it_restarts, it_task, clk_head, clk_wait, clk_tail;
 };
 
 CFB_HD int popc64(uint64_t x) {

@@ -195,6 +195,14 @@ extern "C" int cfb_ctx_request_breakdown(cfb_ctx* c, uint64_t out[8]) {
 	out[3] = h.w8_try_row; out[4] = h.w8_ok_row; out[5] = h.w8_try_range; out[6] = h.w8_ok_range; out[7] = h.w8_ok_w5;
 	return CFB_OK;
 }
+extern "C" int cfb_ctx_search_iter_stats(cfb_ctx* c, uint64_t out[8]) {
+	if(!c || !out) return fail(CFB_EINVAL, "null argument");
+	CK(cudaSetDevice(c->ix->device));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	out[0] = h.it_warp; out[1] = h.it_lane_req; out[2] = h.it_consumers; out[3] = h.it_restarts; out[4] = h.it_task;
+	out[5] = h.clk_head; out[6] = h.clk_wait; out[7] = h.clk_tail;
+	return CFB_OK;
+}
 
 __device__ __forceinline__ uint64_t gmix(uint64_t x) { x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31); }
 // independent, uniformly random gathers of W 8-byte words per request from array `a` of `n` requests' worth, `iters` x ILP per thread
@@ -218,8 +226,9 @@ __global__ void __launch_bounds__(128) k_gather_probe(const unsigned long long* 
 }
 // table: 0 = rank16 (16-byte entries), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it),
 // 4 = death bits, which have no table of their own (always "not built")
-extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_requests, double* g_requests_per_s, double* ms_out) {
-	if(!ix || !g_requests_per_s || ix->device < 0) return fail(CFB_EINVAL, "cfb_gather_ceiling: bad argument");
+// ctas_per_sm CTAs of 128 threads per SM (all resident when <= 16), ilp independent requests per thread in flight
+extern "C" int cfb_gather_rate(const cfb_index* ix, int table, uint64_t n_requests, int ctas_per_sm, int ilp, double* g_requests_per_s, double* ms_out) {
+	if(!ix || !g_requests_per_s || ix->device < 0 || ctas_per_sm < 1 || (ilp != 1 && ilp != 2 && ilp != 4)) return fail(CFB_EINVAL, "cfb_gather_rate: bad argument");
 	CK(cudaSetDevice(ix->device));
 	const cfb_index_tables& t = ix->tables; const IndexView& v = ix->view;
 	const unsigned long long* base = nullptr; uint64_t n = 0; int W = 1;
@@ -229,17 +238,18 @@ extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_req
 		case 2: base = (const unsigned long long*)v.walk8; n = t.walk8_bytes / 8; W = 1; break;
 		case 3: base = v.rtab32 ? (const unsigned long long*)v.rtab32 : (const unsigned long long*)v.rtab16; n = t.resolve_table_bytes / 8; W = 1; break;
 		case 4: break;      // death bits: no table of their own, they live in the K-mer table's entries
-		default: return fail(CFB_EINVAL, "cfb_gather_ceiling: unknown table %d", table);
+		default: return fail(CFB_EINVAL, "cfb_gather_rate: unknown table %d", table);
 	}
-	if(!base || n == 0) return fail(CFB_EINVAL, "cfb_gather_ceiling: table %d is not built", table);
-	const int ILP = 4, threads = 128;
-	const int blocks = ix->sm_count * 16;
-	const uint64_t per_iter = (uint64_t)blocks * threads * ILP;
+	if(!base || n == 0) return fail(CFB_EINVAL, "cfb_gather_rate: table %d is not built", table);
+	const int threads = 128;
+	const int blocks = ix->sm_count * ctas_per_sm;
+	const uint64_t per_iter = (uint64_t)blocks * threads * ilp;
 	const uint32_t iters = (uint32_t)std::max<uint64_t>(1, n_requests / per_iter);
 	unsigned long long* sink = nullptr; CK(cudaMalloc((void**)&sink, 8));
 	cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
 	auto launch = [&](uint32_t it) {
-		if(W == 2) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink);
+		if(W == 2) { if(ilp == 4) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink); else if(ilp == 2) k_gather_probe<2, 2><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<2, 1><<<blocks, threads>>>(base, n, it, sink); }
+		else { if(ilp == 4) k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink); else if(ilp == 2) k_gather_probe<1, 2><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<1, 1><<<blocks, threads>>>(base, n, it, sink); }
 	};
 	launch(std::max<uint32_t>(1, iters / 16)); CK(cudaDeviceSynchronize());      // warm-up
 	CK(cudaEventRecord(e0)); launch(iters); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
@@ -249,4 +259,8 @@ extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_req
 	*g_requests_per_s = (double)per_iter * iters / ((double)ms * 1e6);
 	if(ms_out) *ms_out = ms;
 	return CFB_OK;
+}
+// the ceiling: 16 CTAs per SM x 4 requests per thread = 8192 requests in flight per SM
+extern "C" int cfb_gather_ceiling(const cfb_index* ix, int table, uint64_t n_requests, double* g_requests_per_s, double* ms_out) {
+	return cfb_gather_rate(ix, table, n_requests, 16, 4, g_requests_per_s, ms_out);
 }

@@ -265,6 +265,14 @@ int cfb_ctx_requests(cfb_ctx*, uint64_t out[5]);
  * range, taken from a range of width >= 5}.  A separate call, so that the sum of cfb_ctx_requests stays the total request count. */
 int cfb_ctx_request_breakdown(cfb_ctx*, uint64_t out[8]);
 int cfb_gather_ceiling(const cfb_index*, int table, uint64_t n_requests, double* g_requests_per_s, double* ms);
+/* The same probe with a chosen number of requests in flight: ctas_per_sm CTAs of 128 threads per SM, ilp (1, 2 or 4) independent
+ * requests per thread.  cfb_gather_ceiling is (16, 4); the search kernel's own shape is (8, 1). */
+int cfb_gather_rate(const cfb_index*, int table, uint64_t n_requests, int ctas_per_sm, int ilp, double* g_requests_per_s, double* ms);
+/* How the search kernel's loop spent its trips in the last batch (CFB_COUNT=2): {warp-iterations, lane-iterations that issued a
+ * table request, consumer branches with at least one lane summed over warp-iterations, restart blocks (hit store, task hand-out,
+ * search start) with at least one lane summed likewise, warp-iterations in which a lane received a task, SM clocks summed over
+ * one lane per warp from the loop top to the fetch issue, from there until the loaded data is usable, from there to the end of the trip}. */
+int cfb_ctx_search_iter_stats(cfb_ctx*, uint64_t out[8]);
 
 /* Operation counters of the last batch on this ctx when it was created with CFB_COUNT=1, which searches with the scalar,
  * table-free restatement of the reference's walk (same definition as SURVEY.md 8d):
