@@ -338,6 +338,16 @@ class Context:
         names = ["warp_iters", "lane_requests", "consumer_paths", "restart_paths", "task_iters", "clk_head", "clk_wait", "clk_tail"]
         return dict(zip(names, [int(x) for x in out]))
 
+    def score_stats(self):
+        """how k_score spent the last batch (CFB_COUNT=1 or 2): totals, and units by rows / by distinct ids in log2 buckets"""
+        out = (C.c_uint64 * 23)()
+        _ck(lib().cfb_ctx_score_stats(self.h, out))
+        v = [int(x) for x in out]
+        names = ["units", "rows", "distinct_ids", "reduce_units", "reduce_rounds", "warps", "warps_global"]
+        d = dict(zip(names, v[:7]))
+        d["rows_hist"], d["distinct_ids_hist"] = v[7:15], v[15:23]
+        return d
+
     def counters(self):
         out = (C.c_uint64 * 8)()
         _ck(lib().cfb_ctx_counters(self.h, out))

@@ -32,8 +32,16 @@ static const uint32_t kBwNone = 0xffffffffu;       // BWTHit::reset(): _bwoff = 
 // Device/host view of the index.  Only lineRate 7 (128-byte sides: 96 B of 2-bit BWT = 384
 // bases, then occ[A,C,G,T] as 4 x u64 counted before the side) is supported by the kernels.
 // ----------------------------------------------------------------------------------------
+// What scoring needs of one sequence id under a context's parameters, in one aligned 16-byte record (see seq_info_of).
+struct alignas(16) SeqInfo {
+	uint64_t taxid;       // after the class_rank_slot resolution
+	int32_t  pid;         // path id or -1 (empty path)
+	uint32_t flags;       // kSeqExcluded | rank the resolution stopped at << 8
+};
+static const uint32_t kSeqExcluded = 1u;
+
 struct IndexView {
-	const uint64_t* sides;      // num_sides * 16 u64: the host twin's; the device replica frees them once rank16 is built (null)
+	const uint64_t* sides;     // num_sides * 16 u64: the host twin's; the device replica frees them once rank16 is built (null)
 	const uint64_t* ftab;
 	const uint64_t* eftab;
 	const uint16_t* sample16;   // exactly one of sample16/sample32 is non-null
@@ -44,8 +52,9 @@ struct IndexView {
 	const uint64_t* seq_taxid;
 	const int32_t*  seq_path;
 	const uint64_t* paths;      // n_paths * 10
-	const uint8_t*  seq_excluded;   // per-sequence flag (per ctx; may be null)
+	const uint8_t*  seq_excluded;   // per-sequence flag (host views only: the device reads it through `seqs`; may be null)
 	const uint64_t* host_taxids;    // sorted expanded host set (per ctx)
+	const SeqInfo*  seqs;           // per ctx: seq_info_of every sequence id (null: computed from the arrays above)
 	const uint64_t* rank16;         // device-only rank entries: 16 bytes (occ_c, 64 indicator bits) per (64 rows, base); format and decoders below
 	const uint64_t* ftab2;          // device-only fused ftab: (top, bot) per 10-mer, eftab already resolved
 	const uint16_t* rtab16;         // device-only resolve table: sequence id of EVERY SA row (one of rtab16/rtab32, or neither)
@@ -89,6 +98,11 @@ struct Counters {   // algorithmic-operation counters (SURVEY.md section 8d defi
 	// summed over warp-iterations, warp-iterations in which a lane received a task, and SM clocks summed by lane 0 over
 	// loop top -> fetch issue, fetch issue -> loaded data usable, loaded data usable -> end of the trip
 	unsigned long long it_warp, it_lane_req, it_consumers, it_restarts, it_task, clk_head, clk_wait, clk_tail;
+	// how k_score spends a batch (count modes 1 and 2): units with rows to score, their rows, their distinct ids (hit-map
+	// entries), units that enter the tree reduction and the rank rounds they run, warps with rows and warps whose rows did not
+	// fit the shared pool (global scratch); rows and distinct ids per unit in log2 buckets (0: 1, 1: 2-3, ..., 7: >= 128)
+	unsigned long long sc_units, sc_rows, sc_nmap, sc_reduce, sc_rounds, sc_warps, sc_warps_global;
+	unsigned long long sc_rows_hist[8], sc_nmap_hist[8];
 };
 
 CFB_HD int popc64(uint64_t x) {
@@ -523,8 +537,12 @@ struct EmitRows {       // second pass: write the SA rows to resolve, in consump
 static const uint32_t kUidOff = 0xffffffffu;
 struct Entry {          // HitCount classifier.h:31-57 (fields that influence output)
 	uint64_t taxID;
+	union {
+		uint32_t scores[2][2];
+		uint64_t parent;     // once reduce_and_emit has summed the scores: the entry's parent in the current rank round of the tree reduction
+	};
+	uint32_t lens[2][2];
 	uint32_t uniqueID;
-	uint32_t scores[2][2], lens[2][2];
 	uint32_t score, hitlen, ts;
 	int32_t  pid;        // path id or -1 (empty path)
 	uint8_t  rank;
@@ -541,7 +559,35 @@ CFB_HD bool is_host(const IndexView& v, uint64_t taxid) {
 	return lo < v.n_host && v.host_taxids[lo] == taxid;
 }
 CFB_HD uint32_t path_size(const Entry& e) { return e.pid < 0 ? 0u : 10u; }
-CFB_HD uint64_t path_at(const IndexView& v, const Entry& e, uint32_t i) { return v.paths[(uint64_t)e.pid * 10 + i]; }
+CFB_HD uint64_t path_at(const IndexView& v, const Entry& e, uint32_t i) {
+#ifdef __CUDA_ARCH__
+	return __ldg(v.paths + (uint64_t)e.pid * 10 + i);      // read-only for the kernel's life: the loads of a loop may overlap its stores
+#else
+	return v.paths[(uint64_t)e.pid * 10 + i];
+#endif
+}
+
+// The record of sequence id `ref` under the context's parameters (score_plan's view of a resolved id): its taxID, or with
+// --classification-rank the first non-zero taxID of its path from class_rank_slot on, its path id, whether the exclude set
+// holds it, and the rank the resolution stopped at.  With rank > 0 and an empty path the reference's loop
+// `for(; rank < path.size(); ...)` does not run and rank keeps its configured value.  cfb_ctx_create tabulates it (IndexView::seqs).
+CFB_HD SeqInfo seq_info_of(const IndexView& v, const Params& p, uint32_t ref) {
+	SeqInfo s; s.taxid = 0; s.pid = -1;
+	uint32_t rank = p.class_rank_slot & 0xffu, excl = 0;
+	if(ref < v.n_seqs) {
+		s.taxid = v.seq_taxid[ref]; s.pid = v.seq_path[ref];
+		excl = v.seq_excluded && v.seq_excluded[ref] ? kSeqExcluded : 0u;
+		if(rank > 0 && s.pid >= 0) {
+			for(; rank < 10; rank++) { const uint64_t t = v.paths[(uint64_t)s.pid * 10 + rank]; if(t != 0) { s.taxid = t; break; } }
+		}
+	}
+	s.flags = excl | rank << 8;
+	return s;
+}
+CFB_HD SeqInfo seq_info(const IndexView& v, const Params& p, uint32_t ref) {
+	if(v.seqs && ref < v.n_seqs) return v.seqs[ref];        // one 16-byte load
+	return seq_info_of(v, p, ref);
+}
 
 // Third pass: consume the resolved ids along the plan carried by the row words, build the hit map
 // (classifier.h:299-345 + addHitToHitMap :982-1050).  Time stamps are non-decreasing along the plan, so "same as the
@@ -561,13 +607,9 @@ CFB_HDN uint32_t score_plan(const IndexView& v, const Params& p, const uint64_t*
 			bool dup = false;                       // coord_ids de-duplication, first-seen order
 			for(uint64_t q = 0; q < e; q++) if(my[q] == ref) { dup = true; break; }
 			if(dup) continue;
-			uint64_t taxID = ref < v.n_seqs ? v.seq_taxid[ref] : 0;
-			if(v.seq_excluded && ref < v.n_seqs && v.seq_excluded[ref]) continue;
-			const int32_t pid = ref < v.n_seqs ? v.seq_path[ref] : -1;
-			uint8_t rank = (uint8_t)p.class_rank_slot;
-			if(rank > 0 && pid >= 0) {
-				for(; rank < 10; rank++) { const uint64_t t = v.paths[(uint64_t)pid * 10 + rank]; if(t != 0) { taxID = t; break; } }
-			}
+			const SeqInfo si = seq_info(v, p, ref);
+			if(si.flags & kSeqExcluded) continue;
+			const uint64_t taxID = si.taxid; const int32_t pid = si.pid; const uint8_t rank = (uint8_t)(si.flags >> 8);
 			uint32_t idx = 0;
 			for(; idx < nmap; ++idx) {
 				const bool same = rank == 0 ? (ref == map[idx].uniqueID) : (taxID == map[idx].taxID);
@@ -589,13 +631,12 @@ CFB_HDN uint32_t score_plan(const IndexView& v, const Params& p, const uint64_t*
 	return nmap;
 }
 
-// rank > 0 with an empty path: the reference's loop `for(; rank < path.size(); ...)` does not
-// run and rank keeps its configured value; handled above because pid < 0 skips the loop.
-
 // finalize + host rule + tree reduction + emit (classifier.h:380-571).
-// map/nmap: hit map; tc: scratch of >= nmap TaxCnt; out: >= nmap records.  Returns #records.
+// map/nmap: hit map; tc: scratch of >= nmap TaxCnt; out: >= nmap records.  Returns #records; *rounds (when given) receives
+// the number of rank rounds the tree reduction ran (0: it did not run).
 CFB_HDN uint32_t reduce_and_emit(const IndexView& v, const Params& p, bool paired, Entry* map, uint32_t nmap,
-                                 TaxCnt* tc, OutRec* out) {
+                                 TaxCnt* tc, OutRec* out, uint32_t* rounds = nullptr) {
+	if(rounds) *rounds = 0;
 	const uint32_t k = p.khits;
 	for(uint32_t i = 0; i < nmap; i++) {
 		Entry& h = map[i];
@@ -621,15 +662,22 @@ CFB_HDN uint32_t reduce_and_emit(const IndexView& v, const Params& p, bool paire
 		if(!p.tree_traverse && nmap > k) return 0;
 		uint8_t rank = 0;
 		while(nmap > k) {
-			uint32_t ntc = 0;
+			if(rounds) *rounds += 1;
+			// every entry of this round gets its parent once, with loads that do not wait for each other; the tc loop below
+			// compares against the stored value
 			for(uint32_t i = 0; i < nmap; i++) {
 				Entry& h = map[i];
 				while(h.rank < rank) {
 					if((uint32_t)h.rank + 1 >= path_size(h)) { h.rank = 255; break; }
 					h.rank += 1; h.taxID = path_at(v, h, h.rank);
 				}
-				if(h.rank > rank) continue;
-				const uint64_t parent = ((uint32_t)rank + 1 >= path_size(h)) ? 1 : path_at(v, h, rank + 1);
+				if(h.rank == rank) h.parent = ((uint32_t)rank + 1 >= path_size(h)) ? 1 : path_at(v, h, rank + 1);
+			}
+			uint32_t ntc = 0;
+			for(uint32_t i = 0; i < nmap; i++) {
+				const Entry& h = map[i];
+				if(h.rank != rank) continue;
+				const uint64_t parent = h.parent;
 				if(parent == 0) continue;
 				uint32_t j = 0;
 				for(; j < ntc; j++) if(tc[j].parent == parent) { tc[j].count += 1; break; }
@@ -644,9 +692,7 @@ CFB_HDN uint32_t reduce_and_emit(const IndexView& v, const Params& p, bool paire
 				const uint64_t parent = tc[j].parent;
 				for(uint32_t i = 0; i < nmap; i++) {
 					Entry& h = map[i];
-					if(h.rank != rank) continue;
-					const uint64_t cur_parent = ((uint32_t)rank + 1 >= path_size(h)) ? 1 : path_at(v, h, rank + 1);
-					if(parent == cur_parent) { h.uniqueID = kUidOff; h.rank = rank + 1; h.taxID = parent; }
+					if(h.rank == rank && h.parent == parent) { h.uniqueID = kUidOff; h.rank = rank + 1; h.taxID = parent; }
 				}
 				bool first = true;
 				for(uint32_t i = 0; i < nmap; i++) {

@@ -203,6 +203,14 @@ extern "C" int cfb_ctx_search_iter_stats(cfb_ctx* c, uint64_t out[8]) {
 	out[5] = h.clk_head; out[6] = h.clk_wait; out[7] = h.clk_tail;
 	return CFB_OK;
 }
+extern "C" int cfb_ctx_score_stats(cfb_ctx* c, uint64_t out[23]) {
+	if(!c || !out) return fail(CFB_EINVAL, "null argument");
+	CK(cudaSetDevice(c->ix->device));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	out[0] = h.sc_units; out[1] = h.sc_rows; out[2] = h.sc_nmap; out[3] = h.sc_reduce; out[4] = h.sc_rounds; out[5] = h.sc_warps; out[6] = h.sc_warps_global;
+	for(int i = 0; i < 8; i++) { out[7 + i] = h.sc_rows_hist[i]; out[15 + i] = h.sc_nmap_hist[i]; }
+	return CFB_OK;
+}
 
 __device__ __forceinline__ uint64_t gmix(uint64_t x) { x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31); }
 // independent, uniformly random gathers of W 8-byte words per request from array `a` of `n` requests' worth, `iters` x ILP per thread

@@ -3,6 +3,7 @@
 #include "../../include/cfb200.h"
 #include "cf_index.h"
 #include "cf_kernels.cuh"
+#include <cub/cub.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -761,16 +762,20 @@ __global__ void __launch_bounds__(128, MINB) k_prep(const UnitArgs a) {
 }
 
 // k_prep hands out row slices per warp, so the rows of a warp's 32 units form one contiguous span.  A warp whose span fits
-// what is left of its CTA's pool stages the span's rows and ids there with coalesced loads; each unit keeps its hit map,
-// TaxCnt scratch and records at its own offset inside the span (nmap <= n bounds them), and the warp stores the records
-// coalesced.  A warp whose span does not fit uses the global scratch at the units' row offsets.
+// what is left of its CTA's pool keeps its units' hit maps there, each at the unit's own offset inside the span (nmap <= n
+// bounds them); a warp whose span does not fit keeps them in the global scratch at the units' row offsets.  Only the hit maps
+// live in the pool: rows and ids are read where k_prep and k_lookup left them, records go straight to the sparse buffer, and the
+// tree reduction's TaxCnt scratch (a fraction of a percent of the units run it) is always the global one.  A span averages
+// ~80 rows on the bench batch (2.4 rows per unit), so what decides how many warps the pool takes is the bytes per row.
 static const int kScoreThreads = 128;
-static const uint32_t kScorePool = 128;       // rows per CTA, 116 bytes each (row, id, Entry, TaxCnt, OutRec); 256 made k_score faster but slowed e2e, where it shares SMs with search kernels (measured)
+static const uint32_t kScorePool = 232;       // hit-map entries per CTA: 14.5 KB, as much shared memory as the earlier pool of 128 rows of 116 bytes, which 256 rows (29 KB) beat in k_score but lost to in e2e, where k_score shares SMs with search kernels (measured)
 static const uint32_t kNoSlot = 0xffffffffu;
-template <int MINB>
+__device__ __forceinline__ uint32_t log2_bucket(uint64_t x) { const uint32_t b = 63u - (uint32_t)__clzll((long long)x); return b < 7u ? b : 7u; }     // x >= 1
+// COUNT: the instantiation of the counting passes, which also fills the sc_* counters (how the rows, distinct ids and tree
+// reductions of the batch are distributed, and how many warps the shared pool could not take)
+template <int MINB, bool COUNT>
 __global__ void __launch_bounds__(kScoreThreads, MINB) k_score(const UnitArgs a) {
-	__shared__ uint64_t s_rows[kScorePool]; __shared__ uint32_t s_ids[kScorePool];
-	__shared__ Entry s_map[kScorePool]; __shared__ TaxCnt s_tc[kScorePool]; __shared__ OutRec s_recs[kScorePool];
+	__shared__ Entry s_map[kScorePool];
 	__shared__ uint32_t s_used;
 	if(threadIdx.x == 0) s_used = 0;
 	__syncthreads();
@@ -793,35 +798,24 @@ __global__ void __launch_bounds__(kScoreThreads, MINB) k_score(const UnitArgs a)
 	}
 	slot = __shfl_sync(0xffffffffu, slot, 0);
 	const bool sh = slot != kNoSlot;
-	if(sh) {
-		for(uint32_t j = lane; j < (uint32_t)span; j += 32) { s_rows[slot + j] = a.rows[base + j]; s_ids[slot + j] = a.ids[base + j]; }
-		__syncwarp();
-	}
-	const uint32_t loc = sh ? slot + (uint32_t)(off - base) : 0u;
 	uint32_t no = 0;
 	if(n > 0) {
 		const uint8_t fl = a.b.flags ? a.b.flags[unit] : 3;
 		int mates = 0;
 		for(int m = 0; m < a.b.n_mates; m++) if(((fl >> m) & 1) && (m ? a.b.len[1][unit] : a.b.len[0][unit]) != 0) mates++;
-		const uint64_t* rows = sh ? s_rows + loc : a.rows + off;
-		const uint32_t* ids = sh ? s_ids + loc : a.ids + off;
-		Entry* map = sh ? s_map + loc : a.entries + off;
-		TaxCnt* tc = sh ? s_tc + loc : a.tcs + off;
-		OutRec* out = sh ? s_recs + loc : a.recs_sparse + off;
-		const uint32_t nmap = score_plan(a.v, a.p, rows, ids, n, map);
-		no = reduce_and_emit(a.v, a.p, mates == 2, map, nmap, tc, out);
-	}
-	if(valid) a.nout[unit] = no;
-	if(sh) {        // each unit's records, three 8-byte words apiece, stored by the whole warp
-		__syncwarp();
-		for(int u = 0; u < 32; u++) {
-			const uint32_t cnt = __shfl_sync(0xffffffffu, no, u) * 3u, l = __shfl_sync(0xffffffffu, loc, u);
-			const uint64_t o = __shfl_sync(0xffffffffu, off, u);
-			const uint64_t* src = reinterpret_cast<const uint64_t*>(s_recs + l);
-			uint64_t* dst = reinterpret_cast<uint64_t*>(a.recs_sparse + o);
-			for(uint32_t w = lane; w < cnt; w += 32) dst[w] = src[w];
+		Entry* map = sh ? s_map + slot + (uint32_t)(off - base) : a.entries + off;
+		const uint32_t nmap = score_plan(a.v, a.p, a.rows + off, a.ids + off, n, map);
+		uint32_t rounds = 0;
+		no = reduce_and_emit(a.v, a.p, mates == 2, map, nmap, a.tcs + off, a.recs_sparse + off, COUNT ? &rounds : nullptr);
+		if(COUNT) {
+			atomicAdd(&a.ctr->sc_units, 1ull); atomicAdd(&a.ctr->sc_rows, (unsigned long long)n); atomicAdd(&a.ctr->sc_nmap, (unsigned long long)nmap);
+			atomicAdd(&a.ctr->sc_rows_hist[log2_bucket(n)], 1ull);
+			if(nmap) atomicAdd(&a.ctr->sc_nmap_hist[log2_bucket(nmap)], 1ull);
+			if(rounds) { atomicAdd(&a.ctr->sc_reduce, 1ull); atomicAdd(&a.ctr->sc_rounds, (unsigned long long)rounds); }
 		}
 	}
+	if(COUNT && lane == 0 && span) { atomicAdd(&a.ctr->sc_warps, 1ull); if(!sh) atomicAdd(&a.ctr->sc_warps_global, 1ull); }
+	if(valid) a.nout[unit] = no;
 }
 
 // =======================================================================================
@@ -986,6 +980,8 @@ __global__ void __launch_bounds__(256) k_lookup(const ResolveArgs a) {
 // =======================================================================================
 // k_compact
 // =======================================================================================
+// thread per unit: every lane's loads are issued together (a warp walking its units one after another measured 0.189 against
+// 0.109 ms per 2 M-unit window on the bench batch)
 __global__ void __launch_bounds__(128) k_compact(uint32_t n_units, const uint64_t* row_off, const uint64_t* out_off,
                                                  const OutRec* sparse, OutRec* dense, uint32_t* rec_off32, uint64_t dense_cap, unsigned int* overflow) {
 	const uint32_t unit = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1288,7 +1284,7 @@ struct Slot {
 	DBuf<uint64_t> pk; DBuf<uint32_t> nm;
 	DBuf<HitRec> hits; DBuf<uint32_t> nhits; DBuf<HitRec> regen; DBuf<uint32_t> regen_n; uint64_t regen_slots = 0; uint32_t full_cap = 0; DBuf<uint32_t> nrows; DBuf<uint64_t> row_off; DBuf<uint64_t> bsum;
 	DBuf<uint64_t> rows; DBuf<uint32_t> ids; DBuf<Entry> entries; DBuf<TaxCnt> tcs; DBuf<OutRec> sparse;
-	DBuf<uint32_t> nout; DBuf<uint64_t> out_off; DBuf<OutRec> dense; DBuf<uint32_t> rec_off32;
+	DBuf<uint32_t> nout; DBuf<uint64_t> out_off; DBuf<uint8_t> scan_tmp; DBuf<OutRec> dense; DBuf<uint32_t> rec_off32;
 	DBuf<unsigned long long> scal;    // [0] search task ctr (u32 used), [1] resolve ctr, [2] overflow, [3] total rows, [4] total recs
 	HBuf<unsigned long long> h_scal;
 	HBuf<OutRec> h_recs; HBuf<uint32_t> h_rec_off;
@@ -1302,7 +1298,7 @@ struct Slot {
 		h_bases.release(); h_off.release(); h_len.release(); h_flags.release(); d_bases.release(); d_off.release(); d_len.release(); d_flags.release();
 		h_words.release(); d_words.release(); d_npos.release(); d_woff.release(); d_wlen.release();
 		pk.release(); nm.release(); hits.release(); nhits.release(); regen.release(); regen_n.release(); nrows.release(); row_off.release(); bsum.release(); rows.release(); ids.release(); entries.release(); tcs.release();
-		sparse.release(); nout.release(); out_off.release(); dense.release(); rec_off32.release(); scal.release(); h_scal.release(); h_recs.release(); h_rec_off.release(); cnt.release();
+		sparse.release(); nout.release(); out_off.release(); scan_tmp.release(); dense.release(); rec_off32.release(); scal.release(); h_scal.release(); h_recs.release(); h_rec_off.release(); cnt.release();
 		for(int i = 0; i < 6; i++) if(ev[i]) cudaEventDestroy(ev[i]);
 		if(st) cudaStreamDestroy(st);
 	}
@@ -1328,7 +1324,7 @@ struct CountsCtx {
 struct cfb_ctx {
 	const cfb_index* ix = nullptr;
 	IndexView view; Params prm;
-	DBuf<uint8_t> d_excl; DBuf<uint64_t> d_host;
+	DBuf<uint64_t> d_host; DBuf<SeqInfo> d_seqs;
 	Slot slots[kSlots];
 	Counters* d_ctr = nullptr; int count = 0;        // CFB_COUNT: 1 = reference operation counters, 2 = the product's own load requests
 	uint64_t launches = 0;
@@ -1370,7 +1366,7 @@ extern "C" void cfb_ctx_destroy(cfb_ctx* c) {
 	comm_release(c);
 	c->cnt.release();
 	for(int i = 0; i < kSlots; i++) c->slots[i].release();
-	c->d_excl.release(); c->d_host.release();
+	c->d_host.release(); c->d_seqs.release();
 	if(c->d_ctr) cudaFree(c->d_ctr);
 	delete c;
 }
@@ -1394,11 +1390,20 @@ extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx*
 	expand_taxids(h, p->host_taxids, p->n_host_taxids, host);
 	expand_taxids(h, p->excluded_taxids, p->n_excluded_taxids, excl);
 	#define CKC(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { cfb_ctx_destroy(c); return fail(CFB_ECUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); } } while(0)
+	// the exclude set reaches the device only through the sequence table: seq_info_of reads the flags for ids < n_seqs alone
+	std::vector<uint8_t> fl;
 	if(!excl.empty()) {
-		std::vector<uint8_t> fl(h.seq_taxid.size(), 0);
+		fl.assign(h.seq_taxid.size(), 0);
 		for(size_t i = 0; i < fl.size(); i++) fl[i] = excl.count(h.seq_taxid[i]) ? 1 : 0;
-		CKC(c->d_excl.ensure(fl.size())); CKC(cudaMemcpy(c->d_excl.p, fl.data(), fl.size(), cudaMemcpyHostToDevice));
-		c->view.seq_excluded = c->d_excl.p;
+	}
+	{     // seq_info_of every sequence id under this context's rank and exclude set: k_score reads one 16-byte record per distinct id
+		IndexView hv; memset(&hv, 0, sizeof hv);
+		hv.seq_taxid = h.seq_taxid.data(); hv.seq_path = h.seq_path.data(); hv.paths = h.paths.data(); hv.n_seqs = (uint32_t)h.seq_taxid.size();
+		hv.seq_excluded = fl.empty() ? nullptr : fl.data();
+		std::vector<SeqInfo> tab(hv.n_seqs);
+		for(uint32_t i = 0; i < hv.n_seqs; i++) tab[i] = seq_info_of(hv, q, i);
+		CKC(c->d_seqs.ensure(tab.size() + 1)); CKC(cudaMemcpy(c->d_seqs.p, tab.data(), tab.size() * sizeof(SeqInfo), cudaMemcpyHostToDevice));
+		c->view.seqs = c->d_seqs.p;
 	}
 	if(!host.empty()) {
 		std::vector<uint64_t> hv(host.begin(), host.end());
@@ -1667,7 +1672,7 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 		}
 		const uint32_t W = (s.maxlen + 31) / 32 + 1;
 		CK(s.pk.ensure(ntasks * W + 2)); CK(s.nm.ensure(ntasks * W + 2)); CK(s.nrows.ensure(n)); CK(s.row_off.ensure(n + 1));
-		CK(s.bsum.ensure(scan_blocks + 1)); CK(s.nout.ensure(n)); CK(s.out_off.ensure(n + 1)); CK(s.rec_off32.ensure(n + 1));
+		CK(s.bsum.ensure(scan_blocks + 1)); CK(s.nout.ensure(n + 1)); CK(s.out_off.ensure(n + 1)); CK(s.rec_off32.ensure(n + 1));
 		s.rows_cap = std::max<uint64_t>(s.rows_cap, c->rows_cap0 ? c->rows_cap0 : std::max<uint64_t>(n * 12, 4096));
 	}
 	CK(s.rows.ensure(s.rows_cap)); CK(s.ids.ensure(s.rows_cap)); CK(s.entries.ensure(s.rows_cap)); CK(s.tcs.ensure(s.rows_cap)); CK(s.sparse.ensure(s.rows_cap));
@@ -1676,6 +1681,10 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	if(time_it) CK(cudaEventRecord(s.ev[0], s.st));
 	Counters* ctr = c->count ? c->d_ctr : nullptr;
 	if(c->count && stage == 0) CK(cudaMemsetAsync(c->d_ctr, 0, sizeof(Counters), s.st));
+	else if(c->count) {      // a re-run from the row stage scores every unit again: its k_score statistics start over
+		const size_t sc0 = offsetof(Counters, sc_units);
+		CK(cudaMemsetAsync(reinterpret_cast<char*>(c->d_ctr) + sc0, 0, sizeof(Counters) - sc0, s.st));
+	}
 	UnitArgs ua; ua.v = c->view; ua.p = c->prm; ua.b = s.bv; ua.hits = s.hits.p; ua.nhits = s.nhits.p; ua.cap = s.cap;
 	ua.nrows = s.nrows.p; ua.row_off = s.row_off.p; ua.row_total = s.scal.p + 3; ua.rows = s.rows.p; ua.ids = s.ids.p; ua.rows_cap = s.rows_cap;
 	ua.entries = s.entries.p; ua.tcs = s.tcs.p; ua.recs_sparse = s.sparse.p; ua.nout = s.nout.p;
@@ -1710,12 +1719,17 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	else k_resolve_c<false, false><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra);
 	c->launches++;
 	if(time_it) CK(cudaEventRecord(s.ev[3], s.st));
-	k_score<12><<<ublocks, kScoreThreads, 0, s.st>>>(ua); c->launches++;        // <= 40 registers and 15.9 KB of shared memory: 12 CTAs per SM
-	k_scan_sums<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.nout.p, n, s.bsum.p);
-	k_scan_top<<<1, 1024, 0, s.st>>>(s.bsum.p, scan_blocks, (uint64_t*)(s.scal.p + 4));
-	k_scan_apply<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.nout.p, n, s.bsum.p, (const uint64_t*)(s.scal.p + 4), s.out_off.p);
+	if(ctr) k_score<12, true><<<ublocks, kScoreThreads, 0, s.st>>>(ua);
+	else k_score<12, false><<<ublocks, kScoreThreads, 0, s.st>>>(ua);        // <= 40 registers and 14.5 KB of shared memory: 12 CTAs per SM
+	// record offsets: one single-pass scan over the n + 1 counts (the last is 0, so out_off[n] is the total), in 64 bits
+	size_t scan_bytes = 0;
+	CK(cub::DeviceScan::ExclusiveScan(nullptr, scan_bytes, s.nout.p, s.out_off.p, cub::Sum(), (uint64_t)0, (int)(n + 1), s.st));
+	CK(s.scan_tmp.ensure(scan_bytes));
+	CK(cudaMemsetAsync(s.nout.p + n, 0, sizeof(uint32_t), s.st));
+	CK(cub::DeviceScan::ExclusiveScan(s.scan_tmp.p, scan_bytes, s.nout.p, s.out_off.p, cub::Sum(), (uint64_t)0, (int)(n + 1), s.st));
+	CK(cudaMemcpyAsync(s.scal.p + 4, s.out_off.p + n, sizeof(uint64_t), cudaMemcpyDeviceToDevice, s.st));
 	k_compact<<<(unsigned)((n + 1 + 127) / 128), 128, 0, s.st>>>((uint32_t)n, s.row_off.p, s.out_off.p, s.sparse.p, s.dense.p, s.rec_off32.p, s.dense_cap, (unsigned int*)(s.scal.p + 2));
-	c->launches += 4;
+	c->launches += 4;      // k_score, the scan's two kernels, k_compact
 	s.folded = false;
 	if(c->fold_records && !s.is_text) {      // this batch's per-taxon counters, on the device, from the records just written
 		const uint32_t nsp = c->cnt.n;

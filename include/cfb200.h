@@ -273,6 +273,10 @@ int cfb_gather_rate(const cfb_index*, int table, uint64_t n_requests, int ctas_p
  * search start) with at least one lane summed likewise, warp-iterations in which a lane received a task, SM clocks summed over
  * one lane per warp from the loop top to the fetch issue, from there until the loaded data is usable, from there to the end of the trip}. */
 int cfb_ctx_search_iter_stats(cfb_ctx*, uint64_t out[8]);
+/* How the scoring kernel spent the last batch (CFB_COUNT=1 or 2): {units with rows to score, their rows, their distinct ids,
+ * units that entered the tree reduction, rank rounds those ran, warps with rows, warps whose rows did not fit the shared pool},
+ * then units by rows and units by distinct ids in eight log2 buckets each (1, 2-3, 4-7, ..., >= 128). */
+int cfb_ctx_score_stats(cfb_ctx*, uint64_t out[23]);
 
 /* Operation counters of the last batch on this ctx when it was created with CFB_COUNT=1, which searches with the scalar,
  * table-free restatement of the reference's walk (same definition as SURVEY.md 8d):
