@@ -82,13 +82,113 @@ std::vector<std::string> split(const std::string& s, char d) {
 	return v;
 }
 
+static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// ------------------------------------------------------------------------------ gzip input
+// A regular file that starts with 1f 8b 08 is gzip: its bytes are inflated on the device (cfb_gunzip_*, on the first
+// listed device) and everything downstream sees the decompressed bytes.  FIFOs and stdin are read as they are.
+static int g_gz_device = 0;
+struct GzTotals { uint64_t files = 0, st[5] = {0, 0, 0, 0, 0}; double t = 0; };
+static GzTotals g_gz;
+
+static bool gzip_magic(int fd) { unsigned char m[3]; return pread(fd, m, 3, 0) == 3 && m[0] == 0x1f && m[1] == 0x8b && m[2] == 8; }
+
+struct GzReader {        // decompressed bytes of one gzip file
+	std::string path; int fd = -1; cfb_gunzip* g = NULL;
+	std::vector<unsigned char> in; size_t in_lo = 0, in_hi = 0; uint64_t file_off = 0; bool file_eof = false;
+	std::vector<unsigned char> look; size_t look_lo = 0, look_hi = 0;       // read-ahead for peek()
+	bool done = false; double t = 0;
+	std::string err;                                                        // "Error: <file>: <reason>" once something failed
+	bool open(const std::string& p, int fd_) {
+		path = p; fd = fd_;
+		if(cfb_gunzip_create(g_gz_device, 0, &g) != CFB_OK) { err = "Error: " + path + ": " + cfb_last_error(); return false; }
+		in.resize(64u << 20);
+		return true;
+	}
+	void close() {
+		if(g) {
+			uint64_t st[5]; cfb_gunzip_stats(g, st);
+			g_gz.files++; for(int k = 0; k < 5; k++) g_gz.st[k] += st[k]; g_gz.t += t;
+			cfb_gunzip_destroy(g); g = NULL;
+		}
+		if(fd >= 0) ::close(fd);
+		fd = -1;
+	}
+	size_t raw_read(unsigned char* dst, size_t n) {
+		size_t got = 0;
+		while(got < n && !done && err.empty()) {
+			if(!file_eof && in_hi - in_lo < in.size() / 2) {
+				memmove(in.data(), in.data() + in_lo, in_hi - in_lo); in_hi -= in_lo; in_lo = 0;
+				while(in_hi < in.size()) {
+					const ssize_t r = pread(fd, in.data() + in_hi, in.size() - in_hi, (off_t)file_off);
+					if(r < 0) { err = "Error: " + path + ": read failed"; return got; }
+					if(r == 0) { file_eof = true; break; }
+					in_hi += (size_t)r; file_off += (uint64_t)r;
+				}
+			}
+			uint64_t no = 0, nc = 0;
+			const double t0 = now_s();
+			const int rc = cfb_gunzip_run(g, in.data() + in_lo, in_hi - in_lo, file_eof ? 1 : 0, dst + got, n - got, &no, &nc);
+			t += now_s() - t0;
+			if(rc != CFB_OK) { err = "Error: " + path + ": " + cfb_last_error(); return got; }
+			in_lo += nc; got += no;
+			if(no == 0 && nc == 0) {
+				if(file_eof) done = true;
+				else if(in_hi - in_lo == in.size()) in.resize(in.size() * 2);      // one block needs more than the buffer holds
+			}
+		}
+		return got;
+	}
+	size_t read(unsigned char* dst, size_t n) {
+		size_t got = std::min(n, look_hi - look_lo);
+		memcpy(dst, look.data() + look_lo, got); look_lo += got;
+		return got + raw_read(dst + got, n - got);
+	}
+	int peek() {
+		if(look_lo == look_hi) {
+			look.resize(1 << 16); look_lo = 0;
+			look_hi = raw_read(look.data(), look.size());
+		}
+		return look_lo < look_hi ? look[look_lo] : -1;
+	}
+};
+
 // ------------------------------------------------------------------------------ reads
 struct FileIn {       // buffered byte source with one-byte peek
 	FILE* f = NULL; std::vector<unsigned char> buf; size_t pos = 0, end = 0;
-	bool open(const std::string& p) { f = p == "-" ? stdin : fopen(p.c_str(), "rb"); buf.resize(1 << 22); return f != NULL; }
-	bool seek(uint64_t off) { pos = end = 0; return f && f != stdin && fseeko(f, (off_t)off, SEEK_SET) == 0; }
-	void close() { if(f && f != stdin) fclose(f); f = NULL; }
-	inline bool fill() { if(!f) return false; end = fread(buf.data(), 1, buf.size(), f); pos = 0; return end > 0; }
+	GzReader* gz = NULL; std::string path;
+	bool open(const std::string& p) {
+		path = p; buf.resize(1 << 22);
+		if(p != "-") {
+			struct stat st;
+			if(::stat(p.c_str(), &st) == 0 && S_ISREG(st.st_mode)) {
+				const int fd = ::open(p.c_str(), O_RDONLY);
+				if(fd >= 0 && gzip_magic(fd)) {
+					gz = new GzReader();
+					if(!gz->open(p, fd)) { std::cerr << gz->err << std::endl; throw 1; }
+					return true;
+				}
+				if(fd >= 0) ::close(fd);
+			}
+		}
+		f = p == "-" ? stdin : fopen(p.c_str(), "rb"); return f != NULL;
+	}
+	// gzip: inflate again from the start of the file and drop the first `off` decompressed bytes
+	bool seek(uint64_t off) {
+		pos = end = 0;
+		if(gz) {
+			std::vector<unsigned char> skip(1 << 22);
+			while(off) { const size_t r = gz->read(skip.data(), (size_t)std::min<uint64_t>(off, skip.size())); if(!gz->err.empty()) { std::cerr << gz->err << std::endl; throw 1; } if(!r) return false; off -= r; }
+			return true;
+		}
+		return f && f != stdin && fseeko(f, (off_t)off, SEEK_SET) == 0;
+	}
+	void close() { if(gz) { gz->close(); delete gz; gz = NULL; } if(f && f != stdin) fclose(f); f = NULL; }
+	inline bool fill() {
+		if(gz) { end = gz->read(buf.data(), buf.size()); pos = 0; if(!gz->err.empty()) { std::cerr << gz->err << std::endl; throw 1; } return end > 0; }
+		if(!f) return false;
+		end = fread(buf.data(), 1, buf.size(), f); pos = 0; return end > 0;
+	}
 	inline int get() { if(pos == end && !fill()) return -1; return buf[pos++]; }
 	inline int peek() { if(pos == end && !fill()) return -1; return buf[pos]; }
 };
@@ -620,11 +720,10 @@ struct KReport {
 __attribute__((target_clones("avx2", "default")))
 static size_t count_nl(const unsigned char* p, size_t n) { size_t c = 0; for(size_t i = 0; i < n; i++) c += p[i] == '\n'; return c; }
 
-static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
 struct SpanFile {        // one input file of a source, consumed in spans that end at record boundaries
 	int fd = -1; uint64_t file_pos = 0, file_size = 0, span_start = 0; bool eof = false;
 	std::vector<unsigned char> carry;              // bytes after the previous cut
+	GzReader* gz = NULL;                           // gzip file: file_pos counts decompressed bytes
 	bool open(const std::string& p) {
 		// stat before open: opening and closing a FIFO (the `centrifuge` wrapper feeds compressed reads through mkfifo,
 		// centrifuge:470-545) would leave its writer without a reader
@@ -634,9 +733,20 @@ struct SpanFile {        // one input file of a source, consumed in spans that e
 		if(fstat(fd, &st) != 0 || !S_ISREG(st.st_mode)) { ::close(fd); fd = -1; return false; }
 		file_size = (uint64_t)st.st_size;
 		posix_fadvise(fd, 0, 0, POSIX_FADV_SEQUENTIAL);
+		if(gzip_magic(fd)) {
+			gz = new GzReader();
+			const bool ok = gz->open(p, fd);
+			fd = -1;
+			if(!ok) return true;                       // reported by the first fill
+		}
 		return true;
 	}
-	void close() { if(fd >= 0) ::close(fd); fd = -1; }
+	void close() {
+		if(gz) { gz->close(); delete gz; gz = NULL; }
+		if(fd >= 0) ::close(fd);
+		fd = -1;
+	}
+	const std::string& error() const { static const std::string none; return gz ? gz->err : none; }
 	// fill buf (capacity cap) with carry + file bytes up to `want`; returns bytes in buf, line ends in *lines.
 	// The file part is read by `threads` preads in parallel, each counting the line ends of its piece.
 	size_t fill(unsigned char* buf, size_t cap, size_t want, size_t* lines, int threads) {
@@ -644,6 +754,15 @@ struct SpanFile {        // one input file of a source, consumed in spans that e
 		if(n) memcpy(buf, carry.data(), n);
 		span_start = file_pos - n;
 		size_t nl = count_nl(buf, n);
+		if(gz) {
+			const size_t take = n < want ? std::min(want - n, cap - 1 - n) : 0;
+			const size_t got = gz->err.empty() ? gz->read(buf + n, take) : 0;
+			nl += count_nl(buf + n, got); n += got; file_pos += got;
+			if(!gz->err.empty() || gz->peek() < 0) eof = true;
+			if(eof && n > 0 && buf[n - 1] != '\n') { buf[n++] = '\n'; nl++; }
+			*lines = nl;
+			return n;
+		}
 		const uint64_t remain = file_size - file_pos;
 		size_t take = n < want ? (size_t)std::min<uint64_t>(remain, std::min(want - n, cap - 1 - n)) : 0;
 		if(take) {
@@ -674,8 +793,9 @@ struct SpanFile {        // one input file of a source, consumed in spans that e
 		return n;
 	}
 	// the byte that follows the last cut (first carried byte, else the next file byte); -1 at the end of the input
-	int next_byte() const {
+	int next_byte() {
 		if(!carry.empty()) return carry[0];
+		if(gz) return gz->peek();
 		if(file_pos >= file_size) return -1;
 		unsigned char c; return pread(fd, &c, 1, (off_t)file_pos) == 1 ? (int)c : -1;
 	}
@@ -748,6 +868,7 @@ struct TextPipe {
 		for(int d = 0; d < N; d++) for(int i = 0; i < S; i++) free_slots[d].push(i);
 		std::atomic<bool> stop(false);
 		double t_read = 0, t_write = 0;
+		std::string read_err;
 
 		std::thread reader([&] {
 			bool first = true;
@@ -760,6 +881,8 @@ struct TextPipe {
 				Span sp; memset(&sp, 0, sizeof sp); sp.dev = d; sp.slot = s;
 				size_t n[2] = {0, 0}, lines[2] = {0, 0};
 				for(int m = 0; m < nm; m++) n[m] = f[m].fill(buf[m][bi], cap, o.text_block, &lines[m], read_threads);
+				for(int m = 0; m < nm; m++) if(!f[m].error().empty() && read_err.empty()) read_err = f[m].error();
+				if(!read_err.empty()) { t_read += now_s() - t0; break; }                        // gzip input failed: rows so far stand
 				if(n[0] == 0 && (!paired || n[1] == 0)) { t_read += now_s() - t0; break; }      // input exhausted
 				size_t rec = lines[0] / L;
 				bool irregular = f[0].eof && lines[0] % L != 0;
@@ -855,6 +978,7 @@ struct TextPipe {
 		reader.join();
 		rows.close(); writer.join();
 		f[0].close(); f[1].close();
+		if(!read_err.empty()) { std::cerr << read_err << std::endl; rc = -1; }
 		st.t_read += t_read; st.t_write += t_write; st.t_gpu_wait += t_wait; st.t_total += now_s() - t_begin;
 		if(rc < 0) return -1;
 		return fallback ? 1 : 0;
@@ -1316,6 +1440,7 @@ extern "C" int cfb_run(int argc, const char** argv) {
 		if(devs.size() == 1 && devs[0] == -1) { devs.clear(); int n = cfb_device_count(); for(int d = 0; d < n; d++) devs.push_back(d); if(devs.empty()) { std::cerr << "Error: no CUDA device (this build has no CPU fallback)" << std::endl; return 1; } }
 		if(devs.empty()) devs.push_back(o.device);
 		const int N = (int)devs.size();
+		g_gz_device = devs[0];
 		// File-to-file runs are bounded by the file system (tens of M reads/s), far below what the plain kernels
 		// deliver (~180 M reads/s), so the tables that buy the last factor of two on the device (resolve table, walk8:
 		// ~0.75 s per Gbp to build) would only delay the first read.  CFB_FULL_TABLES=1 builds them anyway.
@@ -1462,6 +1587,8 @@ extern "C" int cfb_run(int argc, const char** argv) {
 			          << " bytes out, " << tstats.fallbacks << " fallbacks); record-level reader: " << host_units << " units" << std::endl;
 			std::cerr << "[cfb] text pipeline " << tstats.t_total << " s: reader busy " << tstats.t_read << " s, device wait " << tstats.t_gpu_wait << " s, writer busy " << tstats.t_write << " s, submit " << tstats.t_submit << " s, pinned setup " << tstats.t_setup << " s" << std::endl;
 			if(N > 1) std::cerr << "[cfb] " << N << " devices, per-taxon counters reduced with NCCL" << std::endl;
+			if(g_gz.files) std::cerr << "[cfb] gunzip: " << g_gz.st[0] << " members, " << g_gz.st[1] << " bytes in, " << g_gz.st[2] << " bytes out, " << g_gz.st[3]
+			                         << " chunks, " << g_gz.st[4] << " re-decoded, " << g_gz.t << " s" << std::endl;
 		}
 		if(fo != stdout) fclose(fo); else fflush(stdout);
 		rs.fo = NULL;

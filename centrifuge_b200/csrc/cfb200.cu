@@ -1015,6 +1015,7 @@ static int fail(int code, const char* fmt, ...) {
 #define CK(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) return fail(CFB_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); } while(0)
 
 extern "C" const char* cfb_last_error(void) { return g_err; }
+int cfb_fail_msg(int code, const char* msg) { return fail(code, "%s", msg); }      // for the other translation units (cf_gunzip.cu)
 extern "C" const char* cfb_version(void) { return "cfb200 0.1 (sm_90a)"; }
 
 template <class T> struct DBuf {     // growable device buffer

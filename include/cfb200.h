@@ -32,6 +32,7 @@ extern "C" {
 #define CFB_ENODEV   -4   /* no usable CUDA device (no CPU fallback exists) */
 #define CFB_ECUDA    -5   /* CUDA runtime error, see cfb_last_error() */
 #define CFB_EFORMAT  -6   /* index geometry not supported by the kernels */
+#define CFB_EDATA    -7   /* corrupt or truncated compressed input */
 
 #define CFB_UID_NONE 0xFFFFFFFFu
 
@@ -303,6 +304,42 @@ int cfb_test_host_path(const char* index_base, const char* reads_a, const char* 
 
 const char* cfb_last_error(void);
 const char* cfb_version(void);
+
+/* ---- gzip inflater: RFC 1952 members of RFC 1951 DEFLATE data, decompressed on the device -------------
+ * Byte for byte what zlib produces, for every block type, header flag and member layout (several members, empty ones,
+ * BGZF).  Each member's CRC-32 and ISIZE are checked.  The compressed stream is cut into chunks of `chunk_kb` KB (0 =
+ * CFB_GZ_CHUNK_KB, else 64) that are decoded in parallel from speculated block starts; a wrong guess is decoded again
+ * from the previous chunk's end, so the output never depends on the guesses.  Device memory grows with the chunk size
+ * (a pass covers 512 chunks), not with the stream.  There is no host inflate. */
+typedef struct cfb_gunzip cfb_gunzip;
+int  cfb_gunzip_create(int device, uint32_t chunk_kb, cfb_gunzip** out);
+void cfb_gunzip_destroy(cfb_gunzip*);
+/* Streaming: feed compressed bytes `in` (the unconsumed tail of the previous call first), get up to out_cap decompressed
+ * bytes.  *n_consumed bytes of `in` were used; pass the rest again, followed by more of the file.  in_is_last != 0: `in`
+ * reaches the end of the file.  A call that returns n_out == 0 and n_consumed == 0 needs more input, or with in_is_last
+ * has finished the file.  Corrupt or truncated data (bad header, reserved block type, invalid code, distance before the
+ * start of the member, CRC-32 or ISIZE mismatch, trailing bytes that are not a member) returns CFB_EDATA, and so does
+ * every later call.  Bytes delivered before an error belong to members or passes that decoded without one. */
+int  cfb_gunzip_run(cfb_gunzip*, const void* in, uint64_t n_in, int in_is_last, void* out, uint64_t out_cap,
+                    uint64_t* n_out, uint64_t* n_consumed);
+/* Resume state between two calls when no output is pending (after a call that filled less than out_cap): restore it
+ * into any inflater and feed the file from in_offset to continue with byte out_offset of the decompressed stream. */
+typedef struct {
+	uint64_t in_offset;        /* compressed bytes consumed before this state */
+	uint64_t out_offset;       /* decompressed bytes produced before this state */
+	uint64_t bit;              /* next bit to decode, counted from in_offset */
+	uint64_t hdr_bit;          /* header of the Huffman block being decoded (~0: at a block boundary), from in_offset */
+	uint64_t member_bytes;     /* decompressed bytes of the current member so far */
+	uint32_t crc;              /* their CRC-32 */
+	uint32_t win_len;          /* valid bytes at the end of window */
+	int32_t  phase;            /* 0: before a member header, 1: inside the DEFLATE data, 2: before the trailer */
+	uint32_t members;          /* members completed */
+	uint8_t  window[32768];    /* the last 32 KB of the member's output */
+} cfb_gunzip_state;
+int  cfb_gunzip_get_state(const cfb_gunzip*, cfb_gunzip_state* out);
+int  cfb_gunzip_set_state(cfb_gunzip*, const cfb_gunzip_state* in);
+/* {members completed, compressed bytes consumed, decompressed bytes produced, chunks decoded, chunks re-decoded} */
+int  cfb_gunzip_stats(const cfb_gunzip*, uint64_t out[5]);
 
 /* ---- index builder (libcfb200): GPU construction of `.1-.4.cf` ----------------------------
  * Replaces: centrifuge-build-bin (centrifuge_build.cpp:472-560 -> Ebwt::initFromVector /
