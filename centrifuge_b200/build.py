@@ -21,7 +21,7 @@ NVCC_FLAGS = [
     "-Wno-deprecated-gpu-targets", "-diag-suppress", "1444",
 ]
 
-LIB_SOURCES = ["cfb200.cu", "cf_build.cu", "cf_em.cu", "cf_gunzip.cu", "cf_index.cpp", "cf_host.cpp"]
+LIB_SOURCES = ["cfb200.cu", "cf_build.cu", "cf_em.cu", "cf_gunzip.cu", "cf_bunzip2.cu", "cf_index.cpp", "cf_host.cpp"]
 CLI_SOURCES = ["cf_cli.cpp"]
 
 

@@ -479,6 +479,58 @@ class Gunzip:
             self.h = C.c_void_p()
 
 
+class Bunzip2:
+    """Streaming bzip2 decompressor on a device (cfb_bunzip2_*).  run() takes compressed bytes and returns
+    (decompressed bytes, compressed bytes consumed); errors raise CfbError with the code in .code."""
+
+    def __init__(self, device=0, pass_kb=0):
+        self.h = C.c_void_p()
+        _ck(lib().cfb_bunzip2_create(C.c_int(device), C.c_uint32(pass_kb), C.byref(self.h)))
+
+    def run(self, data, is_last, out_cap=1 << 24):
+        src = np.frombuffer(data, dtype=np.uint8) if len(data) else np.zeros(1, dtype=np.uint8)
+        out = np.empty(max(1, out_cap), dtype=np.uint8)
+        n_out, n_in = C.c_uint64(), C.c_uint64()
+        rc = lib().cfb_bunzip2_run(self.h, src.ctypes.data_as(C.c_void_p), C.c_uint64(len(data)), C.c_int(1 if is_last else 0),
+                                   out.ctypes.data_as(C.c_void_p), C.c_uint64(out_cap), C.byref(n_out), C.byref(n_in))
+        if rc != 0:
+            e = CfbError("cfb200 error %d: %s" % (rc, lib().cfb_last_error().decode()))
+            e.code = rc
+            raise e
+        return out[: n_out.value].tobytes(), int(n_in.value)
+
+    def decompress_iter(self, data, piece=None, out_cap=1 << 24):
+        """Yield the decompressed stream of `data`, fed in pieces of `piece` bytes (all at once when None)."""
+        piece = piece or max(1, len(data))
+        pos, held = 0, b""
+        while True:
+            if pos < len(data) and len(held) < piece:
+                held += data[pos: pos + piece]
+                pos = min(len(data), pos + piece)
+            out, used = self.run(held, pos >= len(data), out_cap)
+            held = held[used:]
+            if out:
+                yield out
+            elif not used:
+                if pos >= len(data):
+                    return
+                held += data[pos: pos + piece]             # the decompressor needs more input than it holds
+                pos = min(len(data), pos + piece)
+
+    def decompress(self, data, piece=None, out_cap=1 << 24):
+        return b"".join(self.decompress_iter(data, piece, out_cap))
+
+    def stats(self):
+        st = (C.c_uint64 * 6)()
+        _ck(lib().cfb_bunzip2_stats(self.h, st))
+        return dict(zip(("streams", "bytes_in", "bytes_out", "blocks", "rejected", "trailing"), (int(x) for x in st)))
+
+    def close(self):
+        if self.h:
+            lib().cfb_bunzip2_destroy(self.h)
+            self.h = C.c_void_p()
+
+
 class BuildOpts(C.Structure):
     _fields_ = [("out_base", C.c_char_p), ("fasta", C.POINTER(C.c_char_p)), ("n_fasta", C.c_int32),
                 ("synth_genera", C.c_uint32), ("synth_species", C.c_uint32), ("synth_len", C.c_uint64), ("synth_seed", C.c_uint64),

@@ -84,24 +84,40 @@ std::vector<std::string> split(const std::string& s, char d) {
 
 static double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
-// ------------------------------------------------------------------------------ gzip input
-// A regular file that starts with 1f 8b 08 is gzip: its bytes are inflated on the device (cfb_gunzip_*, on the first
+// ------------------------------------------------------------------------------ compressed input
+// A regular file that starts with 1f 8b 08 is gzip, one that starts with "BZh" + a level digit + a block or
+// end-of-stream magic is bzip2: its bytes are decompressed on the device (cfb_gunzip_* / cfb_bunzip2_*, on the first
 // listed device) and everything downstream sees the decompressed bytes.  FIFOs and stdin are read as they are.
 static int g_gz_device = 0;
-struct GzTotals { uint64_t files = 0, st[5] = {0, 0, 0, 0, 0}; double t = 0; };
-static GzTotals g_gz;
+struct GzTotals { uint64_t files = 0, st[6] = {0, 0, 0, 0, 0, 0}; double t = 0; };
+static GzTotals g_gz, g_bz;                     // per format: gzip, bzip2
+// One input file (or pair) of the command line can be read twice: in spans, then by the record-level reader from a
+// span that failed.  Its trailing-garbage warning is printed once per such input, keyed by its position in the list.
+static std::atomic<uint64_t> g_input_seq(0);
+static std::mutex g_warn_mu;
+static std::set<std::pair<uint64_t, std::string>> g_warned;
 
-static bool gzip_magic(int fd) { unsigned char m[3]; return pread(fd, m, 3, 0) == 3 && m[0] == 0x1f && m[1] == 0x8b && m[2] == 8; }
+enum { FMT_PLAIN = 0, FMT_GZIP = 1, FMT_BZIP2 = 2 };
+static int compressed_format(int fd) {
+	unsigned char m[10];
+	const ssize_t k = pread(fd, m, 10, 0);
+	if(k >= 3 && m[0] == 0x1f && m[1] == 0x8b && m[2] == 8) return FMT_GZIP;
+	static const unsigned char blk[6] = {0x31, 0x41, 0x59, 0x26, 0x53, 0x59}, eos[6] = {0x17, 0x72, 0x45, 0x38, 0x50, 0x90};
+	if(k == 10 && m[0] == 'B' && m[1] == 'Z' && m[2] == 'h' && m[3] >= '1' && m[3] <= '9' && (!memcmp(m + 4, blk, 6) || !memcmp(m + 4, eos, 6)))
+		return FMT_BZIP2;
+	return FMT_PLAIN;
+}
 
-struct GzReader {        // decompressed bytes of one gzip file
-	std::string path; int fd = -1; cfb_gunzip* g = NULL;
+struct GzReader {        // decompressed bytes of one gzip or bzip2 file
+	std::string path; int fd = -1; cfb_gunzip* g = NULL; cfb_bunzip2* bz = NULL;
 	std::vector<unsigned char> in; size_t in_lo = 0, in_hi = 0; uint64_t file_off = 0; bool file_eof = false;
 	std::vector<unsigned char> look; size_t look_lo = 0, look_hi = 0;       // read-ahead for peek()
-	bool done = false; double t = 0;
+	bool done = false, starved = false; double t = 0;
 	std::string err;                                                        // "Error: <file>: <reason>" once something failed
-	bool open(const std::string& p, int fd_) {
+	bool open(const std::string& p, int fd_, int fmt) {
 		path = p; fd = fd_;
-		if(cfb_gunzip_create(g_gz_device, 0, &g) != CFB_OK) { err = "Error: " + path + ": " + cfb_last_error(); return false; }
+		const int rc = fmt == FMT_BZIP2 ? cfb_bunzip2_create(g_gz_device, 0, &bz) : cfb_gunzip_create(g_gz_device, 0, &g);
+		if(rc != CFB_OK) { err = "Error: " + path + ": " + cfb_last_error(); return false; }
 		in.resize(64u << 20);
 		return true;
 	}
@@ -111,13 +127,24 @@ struct GzReader {        // decompressed bytes of one gzip file
 			g_gz.files++; for(int k = 0; k < 5; k++) g_gz.st[k] += st[k]; g_gz.t += t;
 			cfb_gunzip_destroy(g); g = NULL;
 		}
+		if(bz) {
+			uint64_t st[6]; cfb_bunzip2_stats(bz, st);
+			g_bz.files++; for(int k = 0; k < 6; k++) g_bz.st[k] += st[k]; g_bz.t += t;
+			if(st[5] && err.empty()) {
+				std::lock_guard<std::mutex> lk(g_warn_mu);
+				if(g_warned.insert(std::make_pair(g_input_seq.load(), path)).second)
+					std::cerr << "Warning: " << path << ": trailing garbage after the last bzip2 stream ignored" << std::endl;
+			}
+			cfb_bunzip2_destroy(bz); bz = NULL;
+		}
 		if(fd >= 0) ::close(fd);
 		fd = -1;
 	}
 	size_t raw_read(unsigned char* dst, size_t n) {
 		size_t got = 0;
 		while(got < n && !done && err.empty()) {
-			if(!file_eof && in_hi - in_lo < in.size() / 2) {
+			if(!file_eof && (in_hi - in_lo < in.size() / 2 || starved)) {
+				starved = false;
 				memmove(in.data(), in.data() + in_lo, in_hi - in_lo); in_hi -= in_lo; in_lo = 0;
 				while(in_hi < in.size()) {
 					const ssize_t r = pread(fd, in.data() + in_hi, in.size() - in_hi, (off_t)file_off);
@@ -128,13 +155,17 @@ struct GzReader {        // decompressed bytes of one gzip file
 			}
 			uint64_t no = 0, nc = 0;
 			const double t0 = now_s();
-			const int rc = cfb_gunzip_run(g, in.data() + in_lo, in_hi - in_lo, file_eof ? 1 : 0, dst + got, n - got, &no, &nc);
+			const int rc = bz ? cfb_bunzip2_run(bz, in.data() + in_lo, in_hi - in_lo, file_eof ? 1 : 0, dst + got, n - got, &no, &nc)
+			                  : cfb_gunzip_run(g, in.data() + in_lo, in_hi - in_lo, file_eof ? 1 : 0, dst + got, n - got, &no, &nc);
 			t += now_s() - t0;
 			if(rc != CFB_OK) { err = "Error: " + path + ": " + cfb_last_error(); return got; }
 			in_lo += nc; got += no;
 			if(no == 0 && nc == 0) {
 				if(file_eof) done = true;
-				else if(in_hi - in_lo == in.size()) in.resize(in.size() * 2);      // one block needs more than the buffer holds
+				else {                                      // the decoder needs more than it was given: read more before the next call
+					if(in_hi - in_lo == in.size()) in.resize(in.size() * 2);
+					starved = true;
+				}
 			}
 		}
 		return got;
@@ -163,9 +194,10 @@ struct FileIn {       // buffered byte source with one-byte peek
 			struct stat st;
 			if(::stat(p.c_str(), &st) == 0 && S_ISREG(st.st_mode)) {
 				const int fd = ::open(p.c_str(), O_RDONLY);
-				if(fd >= 0 && gzip_magic(fd)) {
+				const int fmt = fd >= 0 ? compressed_format(fd) : FMT_PLAIN;
+				if(fmt != FMT_PLAIN) {
 					gz = new GzReader();
-					if(!gz->open(p, fd)) { std::cerr << gz->err << std::endl; throw 1; }
+					if(!gz->open(p, fd, fmt)) { std::cerr << gz->err << std::endl; throw 1; }
 					return true;
 				}
 				if(fd >= 0) ::close(fd);
@@ -173,7 +205,7 @@ struct FileIn {       // buffered byte source with one-byte peek
 		}
 		f = p == "-" ? stdin : fopen(p.c_str(), "rb"); return f != NULL;
 	}
-	// gzip: inflate again from the start of the file and drop the first `off` decompressed bytes
+	// gzip / bzip2: decompress again from the start of the file and drop the first `off` decompressed bytes
 	bool seek(uint64_t off) {
 		pos = end = 0;
 		if(gz) {
@@ -723,7 +755,7 @@ static size_t count_nl(const unsigned char* p, size_t n) { size_t c = 0; for(siz
 struct SpanFile {        // one input file of a source, consumed in spans that end at record boundaries
 	int fd = -1; uint64_t file_pos = 0, file_size = 0, span_start = 0; bool eof = false;
 	std::vector<unsigned char> carry;              // bytes after the previous cut
-	GzReader* gz = NULL;                           // gzip file: file_pos counts decompressed bytes
+	GzReader* gz = NULL;                           // gzip or bzip2 file: file_pos counts decompressed bytes
 	bool open(const std::string& p) {
 		// stat before open: opening and closing a FIFO (the `centrifuge` wrapper feeds compressed reads through mkfifo,
 		// centrifuge:470-545) would leave its writer without a reader
@@ -733,9 +765,9 @@ struct SpanFile {        // one input file of a source, consumed in spans that e
 		if(fstat(fd, &st) != 0 || !S_ISREG(st.st_mode)) { ::close(fd); fd = -1; return false; }
 		file_size = (uint64_t)st.st_size;
 		posix_fadvise(fd, 0, 0, POSIX_FADV_SEQUENTIAL);
-		if(gzip_magic(fd)) {
+		if(const int fmt = compressed_format(fd)) {
 			gz = new GzReader();
-			const bool ok = gz->open(p, fd);
+			const bool ok = gz->open(p, fd, fmt);
 			fd = -1;
 			if(!ok) return true;                       // reported by the first fill
 		}
@@ -882,7 +914,7 @@ struct TextPipe {
 				size_t n[2] = {0, 0}, lines[2] = {0, 0};
 				for(int m = 0; m < nm; m++) n[m] = f[m].fill(buf[m][bi], cap, o.text_block, &lines[m], read_threads);
 				for(int m = 0; m < nm; m++) if(!f[m].error().empty() && read_err.empty()) read_err = f[m].error();
-				if(!read_err.empty()) { t_read += now_s() - t0; break; }                        // gzip input failed: rows so far stand
+				if(!read_err.empty()) { t_read += now_s() - t0; break; }                        // compressed input failed: rows so far stand
 				if(n[0] == 0 && (!paired || n[1] == 0)) { t_read += now_s() - t0; break; }      // input exhausted
 				size_t rec = lines[0] / L;
 				bool irregular = f[0].eof && lines[0] % L != 0;
@@ -1509,6 +1541,7 @@ extern "C" int cfb_run(int argc, const char** argv) {
 		if(text_ok) for(int i = 0; i < N; i++) if(cfb_ctx_set_columns(rs.ctx[i], o.cols.spec().c_str()) != CFB_OK) { std::cerr << "Error: " << cfb_last_error() << std::endl; return 1; }
 		for(size_t si = 0; si < srcs.size() && !failed && !stop; si++) {
 			const Src& src = srcs[si];
+			g_input_seq = si + 1;
 			uint64_t off[2] = {0, 0}, cntA = 0, cntB = 0;      // cnt: records of this list read so far (PatternSource::readCnt_)
 			size_t fi = 0;
 			// whole files go through the text operator while they stay regular and the mate files stay in step
@@ -1589,6 +1622,8 @@ extern "C" int cfb_run(int argc, const char** argv) {
 			if(N > 1) std::cerr << "[cfb] " << N << " devices, per-taxon counters reduced with NCCL" << std::endl;
 			if(g_gz.files) std::cerr << "[cfb] gunzip: " << g_gz.st[0] << " members, " << g_gz.st[1] << " bytes in, " << g_gz.st[2] << " bytes out, " << g_gz.st[3]
 			                         << " chunks, " << g_gz.st[4] << " re-decoded, " << g_gz.t << " s" << std::endl;
+			if(g_bz.files) std::cerr << "[cfb] bunzip2: " << g_bz.st[0] << " streams, " << g_bz.st[1] << " bytes in, " << g_bz.st[2] << " bytes out, " << g_bz.st[3]
+			                         << " blocks, " << g_bz.st[4] << " rejected block starts, " << g_bz.t << " s" << std::endl;
 		}
 		if(fo != stdout) fclose(fo); else fflush(stdout);
 		rs.fo = NULL;

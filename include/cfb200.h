@@ -341,6 +341,32 @@ int  cfb_gunzip_set_state(cfb_gunzip*, const cfb_gunzip_state* in);
 /* {members completed, compressed bytes consumed, decompressed bytes produced, chunks decoded, chunks re-decoded} */
 int  cfb_gunzip_stats(const cfb_gunzip*, uint64_t out[5]);
 
+/* ---- bzip2 decompressor: bzip2 streams (one or several concatenated), decompressed on the device -------------------
+ * Byte for byte what `bzip2 -dc` (libbz2 1.0.8) produces, for every level, concatenated and empty streams.  Each block's
+ * CRC and each stream's combined CRC are checked.  Each pass scans `pass_kb` KB of compressed input (0 = CFB_BZ2_PASS_KB,
+ * else 65536) for block starts and decodes the blocks it finds in parallel.  Device memory grows with the blocks a pass
+ * holds, not with the stream: about 4.8 MB per block (BWT column, tt array, segment tables), at most one block per 128 KB
+ * of pass and 512 in all, plus the pass's input and a 64 MB staging buffer (and 64 MB of pinned host memory).  A file
+ * with 512 or more blocks per pass therefore takes about 2.6 GB of device memory at the default pass size (a 16 MB
+ * pass: 128 blocks, about 0.75 GB); a smaller file takes only what its blocks need.  Randomised blocks (obsolete since
+ * bzip2 0.9.5) are rejected, and so is a block that pads one code length with more than 40 +1/-1 steps (no encoder
+ * writes more than 19).  There is no host decoder.  CFB_ENODEV without a device. */
+typedef struct cfb_bunzip2 cfb_bunzip2;
+int  cfb_bunzip2_create(int device, uint32_t pass_kb, cfb_bunzip2** out);
+void cfb_bunzip2_destroy(cfb_bunzip2*);
+/* Streaming, with the contract of cfb_gunzip_run: feed compressed bytes `in` (the unconsumed tail of the previous call
+ * first), get up to out_cap decompressed bytes; *n_consumed bytes of `in` were used.  A call that returns n_out == 0 and
+ * n_consumed == 0 needs more input, or with in_is_last has finished the file.  Bytes after a complete stream that do not
+ * start with "BZh1".."BZh9" are ignored and counted, as `bzip2 -dc` does.  Corrupt or truncated data (bad block header,
+ * invalid selector, code or code length, origPtr out of range, a block longer than its level allows, a block or stream
+ * CRC mismatch, a randomised block) returns CFB_EDATA, and so does every later call.  Bytes are delivered only from
+ * blocks whose CRC has been checked. */
+int  cfb_bunzip2_run(cfb_bunzip2*, const void* in, uint64_t n_in, int in_is_last, void* out, uint64_t out_cap,
+                     uint64_t* n_out, uint64_t* n_consumed);
+/* {streams completed, compressed bytes consumed, decompressed bytes produced, blocks, rejected block starts (block
+ * magics inside other data), trailing bytes ignored} */
+int  cfb_bunzip2_stats(const cfb_bunzip2*, uint64_t out[6]);
+
 /* ---- index builder (libcfb200): GPU construction of `.1-.4.cf` ----------------------------
  * Replaces: centrifuge-build-bin (centrifuge_build.cpp:472-560 -> Ebwt::initFromVector /
  * buildToDisk, bt2_idx.h:1247-1640,3379-3840) for lineRate 7 indexes.  Either FASTA inputs, or
