@@ -348,6 +348,12 @@ class Context:
         d["rows_hist"], d["distinct_ids_hist"] = v[7:15], v[15:23]
         return d
 
+    def long_stats(self):
+        """long units classified by this context so far (cfb_ctx_long_stats)"""
+        out = (C.c_uint64 * 4)()
+        _ck(lib().cfb_ctx_long_stats(self.h, out))
+        return dict(zip(["units", "bases", "segment_searches", "researched"], [int(x) for x in out]))
+
     def counters(self):
         out = (C.c_uint64 * 8)()
         _ck(lib().cfb_ctx_counters(self.h, out))

@@ -1618,6 +1618,10 @@ extern "C" int cfb_run(int argc, const char** argv) {
 			std::cerr << "[cfb] index load " << std::chrono::duration<double>(t_loaded - t_start).count() << " s, reads " << std::chrono::duration<double>(t_done - t_loaded).count() << " s" << std::endl;
 			std::cerr << "[cfb] text operator: " << tstats.units << " units in " << tstats.spans << " spans (" << tstats.bytes_in << " bytes in, " << tstats.bytes_out
 			          << " bytes out, " << tstats.fallbacks << " fallbacks); record-level reader: " << host_units << " units" << std::endl;
+			uint64_t lt[4] = {0, 0, 0, 0};
+			for(cfb_ctx* x : rs.ctx) { uint64_t v[4]; if(cfb_ctx_long_stats(x, v) == CFB_OK) for(int i = 0; i < 4; i++) lt[i] += v[i]; }
+			std::cerr << "[cfb] long units: " << lt[0] << " (" << lt[1] << " bases), " << lt[2] << " partial searches in segment chains, "
+			          << lt[3] << " re-searched at the join" << std::endl;
 			std::cerr << "[cfb] text pipeline " << tstats.t_total << " s: reader busy " << tstats.t_read << " s, device wait " << tstats.t_gpu_wait << " s, writer busy " << tstats.t_write << " s, submit " << tstats.t_submit << " s, pinned setup " << tstats.t_setup << " s" << std::endl;
 			if(N > 1) std::cerr << "[cfb] " << N << " devices, per-taxon counters reduced with NCCL" << std::endl;
 			if(g_gz.files) std::cerr << "[cfb] gunzip: " << g_gz.st[0] << " members, " << g_gz.st[1] << " bytes in, " << g_gz.st[2] << " bytes out, " << g_gz.st[3]

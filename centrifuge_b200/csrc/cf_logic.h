@@ -267,8 +267,89 @@ CFB_HDN uint32_t search_strand_scalar(const IndexView& v, const Params& p, const
 	return n;
 }
 
+// ----------------------------------------------------------------------------------------
+// Segmented chains (units with a mate longer than kLongUnitLen bases).  Where the greedy chain of search_strand_scalar goes
+// after a partial search depends on the position it started at alone (chain_next), so two chains that visit one position
+// agree from there on.  A long strand is cut into segments of `seg` bases; a speculative chain starts at each segment's first
+// base and runs until it reaches a position at or past the next segment's start (seg_chain).  The join then follows the true
+// chain from position 0 (seg_join): wherever it stands on a position the speculative chain of that segment visited, that
+// chain's hits are the true ones up to its exit; elsewhere it runs the partial searches itself.  Every hit records the
+// position its partial search started at (bwoff), so the visited positions of a segment are its hits' bwoffs, ascending.
+// `step(cur, hit, new_cur, done)` is one partial search: partial_search_scalar on the host, the table walk on the device.
+// ----------------------------------------------------------------------------------------
+static const uint32_t kLongUnitLen = 60000;          // units with a longer mate take the segmented path
+static const uint32_t kMaxMateLen = 0x7fffffffu;     // 2^31 - 1: len1 + len2 and a record's summed hit length stay in 32 bits
+static const uint32_t kChainEnd = 0xffffffffu;       // seg_chain's exit when the chain ended inside the segment
+
+// the chain's next start after the hit `h` of the partial search from cur (new_cur, done as it returned); false: the chain ends
+CFB_HD bool chain_next(const Params& p, uint32_t len, const HitRec& h, uint32_t new_cur, bool done, uint32_t& cur) {
+	cur = new_cur;
+	if(done) return false;
+	if(h.len > p.increment) cur += 1;
+	return cur + p.min_hitlen < len;
+}
+
+// The speculative chain from `start`: stores one hit per position it visits below `stop` (at most stop - start hits) and
+// returns their number; *exit receives the first position >= stop it reached, or kChainEnd.
+template <class Step> CFB_HDN uint32_t seg_chain(const Params& p, uint32_t len, uint32_t start, uint32_t stop, Step& step,
+                                                 HitRec* hits, uint32_t* exit) {
+	uint32_t cur = start, n = 0;
+	for(;;) {
+		if(cur >= stop) { *exit = cur; return n; }
+		HitRec h; uint32_t nc; bool done;
+		step(cur, h, nc, done);
+		hits[n++] = h;
+		if(!chain_next(p, len, h, nc, done, cur)) { *exit = kChainEnd; return n; }
+	}
+}
+
+// The true chain of the strand, from the speculative chains of its segments: segment k's hits at shits + k * seg (sn[k] of
+// them, exit sexit[k]).  Writes the hits search_strand_scalar would produce to out (capacity len) and returns their number;
+// *researched counts the partial searches the join ran itself.
+template <class Step> CFB_HDN uint32_t seg_join(const Params& p, uint32_t len, uint32_t seg, const HitRec* shits, const uint32_t* sn,
+                                                const uint32_t* sexit, Step& step, HitRec* out, unsigned long long* researched) {
+	if(len == 0) return 0;
+	uint32_t q = 0, n = 0;
+	for(;;) {
+		const uint32_t k = q / seg, m = sn[k];
+		const HitRec* H = shits + (uint64_t)k * seg;
+		uint32_t lo = 0, hi = m;
+		while(lo < hi) { const uint32_t mid = (lo + hi) >> 1; if(H[mid].bwoff < q) lo = mid + 1; else hi = mid; }
+		if(lo < m && H[lo].bwoff == q) {        // the speculative chain stands here too: it is the true chain up to its exit
+			for(uint32_t i = lo; i < m; i++) out[n++] = H[i];
+			if(sexit[k] == kChainEnd) return n;
+			q = sexit[k];
+		} else {
+			HitRec h; uint32_t nc; bool done;
+			step(q, h, nc, done);
+			*researched += 1;
+			out[n++] = h;
+			if(!chain_next(p, len, h, nc, done, q)) return n;
+		}
+	}
+}
+
 CFB_HD uint64_t bw64(const HitRec& h) { return h.bwoff == kBwNone ? kOff : (uint64_t)h.bwoff; }
 CFB_HD uint64_t hsize(const HitRec& h) { return h.bot - h.top; }
+
+// Trimming of overlapping hits within each strand list (the last part of post_search).
+CFB_HD void trim_lists(HitRec* F, uint32_t nF, HitRec* R, uint32_t nR) {
+	for(int s = 0; s < 2; s++) {
+		HitRec* L = s == 0 ? F : R; const uint32_t n = s == 0 ? nF : nR;
+		if(n < 2) continue;
+		for(uint32_t i = 0; i + 1 < n; i++) {
+			for(uint32_t j = i + 1; j < n; j++) {
+				const uint64_t abw = bw64(L[i]), bbw = bw64(L[j]);
+				if(abw >= bbw) { L[i].len = 0; break; }
+				if(abw + L[i].len <= bbw) break;
+				if(L[i].len >= L[j].len) {
+					const uint64_t e = bbw + L[j].len, nb = abw + L[i].len;
+					L[j].bwoff = (uint32_t)nb; L[j].len = (uint32_t)(e - nb);
+				} else L[i].len = (uint32_t)(bbw - abw);
+			}
+		}
+	}
+}
 
 // Post-search part of searchForwardAndReverse for one mate: extend, twin removal, trim.
 CFB_HDN void post_search(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t rdlen,
@@ -318,21 +399,79 @@ CFB_HDN void post_search(const IndexView& v, const Params& p, const uint8_t* fw,
 			}
 		}
 	}
-	for(int s = 0; s < 2; s++) {
-		HitRec* L = s == 0 ? F : R; const uint32_t n = s == 0 ? nF : nR;
-		if(n < 2) continue;
-		for(uint32_t i = 0; i + 1 < n; i++) {
-			for(uint32_t j = i + 1; j < n; j++) {
-				const uint64_t abw = bw64(L[i]), bbw = bw64(L[j]);
-				if(abw >= bbw) { L[i].len = 0; break; }
-				if(abw + L[i].len <= bbw) break;
-				if(L[i].len >= L[j].len) {
-					const uint64_t e = bbw + L[j].len, nb = abw + L[i].len;
-					L[j].bwoff = (uint32_t)nb; L[j].len = (uint32_t)(e - nb);
-				} else L[i].len = (uint32_t)(bbw - abw);
+	trim_lists(F, nF, R, nR);
+}
+
+// Whether a strand list is a raw greedy chain: every hit non-empty and placed, each one ending at or before the next starts.
+CFB_HD bool is_chain(const HitRec* L, uint32_t n, uint32_t rdlen) {
+	for(uint32_t i = 0; i < n; i++) {
+		if(L[i].bwoff == kBwNone || L[i].len == 0 || (uint64_t)L[i].bwoff + L[i].len > rdlen) return false;
+		if(i + 1 < n && (uint64_t)L[i].bwoff + L[i].len > L[i + 1].bwoff) return false;
+	}
+	return true;
+}
+
+// post_search for the long hit lists of a long unit, without the nF x nR double loops.  On raw chains (is_chain; otherwise this
+// is post_search itself) both loops reduce to the few pairs whose intervals can meet, in the same order:
+//  - In read coordinates R[j] covers [rcl_j, rcr_j) with rcl strictly decreasing in j and rcr_j <= rcl_{j-1}.  An extension of
+//    R[j] moves only its right end (to the r of the F hit that extended it), and an extension of F[i] only its left end, so rcl
+//    stays as it was and every r an earlier F hit had is <= F[i]'s start l.  So at F[i] only R hits whose original interval
+//    meets [l, r) pass the two overlap tests: j from the first with rcl_j < r through the first with rcl_j <= l.
+//  - The twin loop for F[i] leaves at the first j with rcl_j < l (a zeroed R hit neither leaves nor matches), so only the R hit
+//    with rcl_j == l can be its twin.
+// rcl: scratch of nR words.
+CFB_HDN void post_search_long(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t rdlen,
+                              HitRec* F, uint32_t nF, HitRec* R, uint32_t nR, uint32_t* rcl, Counters* ctr) {
+	if(!is_chain(F, nF, rdlen) || !is_chain(R, nR, rdlen)) { post_search(v, p, fw, rdlen, F, nF, R, nR, ctr); return; }
+	const uint64_t minHitLen = p.min_hitlen;
+	uint64_t sum[2] = {0, 0};
+	for(uint32_t i = 0; i < nF; i++) if(F[i].len >= minHitLen) sum[0] += F[i].len;
+	for(uint32_t i = 0; i < nR; i++) if(R[i].len >= minHitLen) sum[1] += R[i].len;
+	if(sum[0] >= minHitLen && sum[1] >= minHitLen) {
+		for(uint32_t j = 0; j < nR; j++) rcl[j] = rdlen - R[j].bwoff - R[j].len;
+		auto first_below = [&](uint64_t x, bool or_equal) -> uint32_t {     // first j with rcl_j < x (or <= x)
+			uint32_t lo = 0, hi = nR;
+			while(lo < hi) { const uint32_t mid = (lo + hi) >> 1; if(rcl[mid] < x || (or_equal && rcl[mid] == x)) hi = mid; else lo = mid + 1; }
+			return lo;
+		};
+		for(uint32_t i = 0; i < nF; i++) {
+			const uint64_t len = F[i].len, l = bw64(F[i]), r = l + len;
+			const uint32_t j1 = first_below(l, true);
+			for(uint32_t j = first_below(r, false); j < nR && j <= j1; j++) {
+				const uint64_t rclen = R[j].len;
+				if(len < minHitLen && rclen < minHitLen) continue;
+				const uint64_t rc_l = (uint64_t)rdlen - bw64(R[j]) - R[j].len, rc_r = rc_l + rclen;
+				if(r <= rc_l) continue;
+				if(rc_r <= l) continue;
+				if(l == rc_l && r == rc_r) continue;
+				if(l < rc_l && r > rc_r) continue;
+				if(l > rc_l && r < rc_r) continue;
+				if(l > rc_l) {
+					HitRec t; uint32_t nc; bool dn;
+					if(ctr) ctr->ext_searches++;
+					partial_search_scalar(v, fw, rdlen, 0, (uint32_t)rc_l, t, nc, dn, ctr);
+					if((uint64_t)t.len == len + l - rc_l) F[i] = t;
+				}
+				if(r > rc_r) {
+					HitRec t; uint32_t nc; bool dn;
+					if(ctr) ctr->ext_searches++;
+					partial_search_scalar(v, fw, rdlen, 1, (uint32_t)((uint64_t)rdlen - r), t, nc, dn, ctr);
+					if((uint64_t)t.len == rclen + r - rc_r) R[j] = t;
+				}
+			}
+		}
+		for(uint32_t i = 0; i < nF; i++) {
+			const uint64_t len = F[i].len, l = bw64(F[i]), r = l + len;
+			const uint32_t j = first_below(l, true);
+			if(j >= nR || rcl[j] != l || R[j].bwoff == kBwNone) continue;
+			const uint64_t rclen = R[j].len, rc_r = l + rclen;
+			if(len == rclen && r == rc_r && hsize(F[i]) + hsize(R[j]) > (uint64_t)p.ihits) {
+				F[i].top = F[i].bot = 0; F[i].bwoff = kBwNone; F[i].len = 0;
+				R[j].top = R[j].bot = 0; R[j].bwoff = kBwNone; R[j].len = 0;
 			}
 		}
 	}
+	trim_lists(F, nF, R, nR);
 }
 
 // strand choice: returns lo | hi<<1 style pair as (first, second)
@@ -513,7 +652,8 @@ struct CountRows {      // same count as SortAndCount on lists that are already 
 
 struct EmitRows {       // second pass: write the SA rows to resolve, in consumption order, with the scoring plan
 	const Params& p; const UnitHits& u; uint64_t* out; uint64_t k; uint32_t ts, last_ts;
-	CFB_HD EmitRows(const Params& p_, const UnitHits& u_, uint64_t* o) : p(p_), u(u_), out(o), k(0), ts(0), last_ts(0xffffffffu) {}
+	uint32_t* hl;           // long units: the whole hit length of every first row (the head keeps 16 bits of it), else null
+	CFB_HD EmitRows(const Params& p_, const UnitHits& u_, uint64_t* o, uint32_t* hl_ = nullptr) : p(p_), u(u_), out(o), k(0), ts(0), last_ts(0xffffffffu), hl(hl_) {}
 	CFB_HD void operator()(int rdi, int fwi, uint64_t maxG) {
 		const HitRec* L = u.L[rdi][fwi]; const uint32_t n = u.n[rdi][fwi];
 		uint64_t cnt = 0;
@@ -525,6 +665,7 @@ struct EmitRows {       // second pass: write the SA rows to resolve, in consump
 			const uint64_t head = kRowStart | ((uint64_t)(L[hi].len & 0xffffu) << 40) | ((uint64_t)(rdi & 1) << 56) | ((uint64_t)(fwi & 1) << 57)
 			                    | (ts == last_ts ? kRowSameTs : 0ull);
 			last_ts = ts;
+			if(hl) hl[k] = L[hi].len;
 			for(uint64_t e = 0; e < nelt; e++) out[k++] = ((L[hi].top + e) & kRowMask) | (e == 0 ? head : 0ull);
 			cnt += nelt;
 			if(cnt >= maxG) break;
@@ -591,13 +732,16 @@ CFB_HD SeqInfo seq_info(const IndexView& v, const Params& p, uint32_t ref) {
 
 // Third pass: consume the resolved ids along the plan carried by the row words, build the hit map
 // (classifier.h:299-345 + addHitToHitMap :982-1050).  Time stamps are non-decreasing along the plan, so "same as the
-// previous hit" (kRowSameTs) reproduces every equality the reference's counter produces.
-CFB_HDN uint32_t score_plan(const IndexView& v, const Params& p, const uint64_t* rows, const uint32_t* ids, uint64_t n, Entry* map) {
+// previous hit" (kRowSameTs) reproduces every equality the reference's counter produces.  WIDE (long units): the hit length of
+// the first row k is hl32[k] (EmitRows' hl), as hits of long reads can exceed the head's 16 bits.
+template <bool WIDE = false>
+CFB_HDN uint32_t score_plan(const IndexView& v, const Params& p, const uint64_t* rows, const uint32_t* ids, uint64_t n, Entry* map,
+                            const uint32_t* hl32 = nullptr) {
 	uint32_t nmap = 0, ts = 0;
 	for(uint64_t k = 0; k < n;) {
 		const uint64_t head = rows[k];
 		if(!(head & kRowSameTs)) ts++;
-		const uint64_t hl = (head >> 40) & 0xffffu; const int rdi = (int)((head >> 56) & 1), fwi = (int)((head >> 57) & 1);
+		const uint64_t hl = WIDE ? (uint64_t)hl32[k] : (head >> 40) & 0xffffu; const int rdi = (int)((head >> 56) & 1), fwi = (int)((head >> 57) & 1);
 		uint64_t nelt = 1;
 		while(k + nelt < n && !(rows[k + nelt] & kRowStart)) nelt++;
 		const uint32_t* my = ids + k; k += nelt;

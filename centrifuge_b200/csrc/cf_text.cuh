@@ -39,9 +39,10 @@ struct TextArgs {
 	uint32_t* nl[2]; const uint64_t* nl_total[2];
 	uint32_t n_rec; int32_t lines_per, n_mates, fasta, trim5, trim3; uint32_t seed;
 	uint32_t* len[2]; uint64_t* off[2]; uint8_t* flags; uint32_t* seedv[2]; uint32_t maxlen_hint;
+	uint32_t keep_long;             // 0: a unit with a mate over kLongUnitLen bases gets flags 0 (the span is run again with the long-unit kernels)
 	uint32_t* name_off; uint32_t* id_len; uint32_t* name_len; uint32_t* seq_off[2]; uint32_t* qual_off[2];
 	uint8_t* bases;
-	unsigned long long* tscal;      // [0] status bits, [1] max length, [2] n_multi, [3] tsv bytes
+	unsigned long long* tscal;      // [0] status bits, [1] max length, [2] n_multi, [3] max length of the mates up to kLongUnitLen bases
 };
 
 // 16-bit mask of bytes equal to `c` in a 16-byte vector
@@ -123,7 +124,10 @@ __global__ void __launch_bounds__(128) k_tok_rec(const TextArgs a) {
 	if(bad) { atomicOr(a.tscal, (unsigned long long)TX_IRREGULAR); return; }
 	const uint32_t len = trimmed_len(nread, a.trim5, a.trim3);
 	if((unsigned long long)len > *(volatile unsigned long long*)(a.tscal + 1)) atomicMax(a.tscal + 1, (unsigned long long)len);   // guarded: one address for all records
-	if(len > a.maxlen_hint) return;            // buffers are sized for the hint: the host re-runs the span with a wider class
+	if(len <= kLongUnitLen && (unsigned long long)len > *(volatile unsigned long long*)(a.tscal + 3)) atomicMax(a.tscal + 3, (unsigned long long)len);
+	// the short kernels' buffers are sized for the hint: the host re-runs the span with a wider class.  Long mates are laid out
+	// by their own lengths, like every mate, and classified by the long-unit kernels.
+	if(len > a.maxlen_hint && len <= kLongUnitLen) return;
 	a.len[m][r] = len;
 	a.seq_off[m][r] = s1; a.qual_off[m][r] = qoff;
 	if(m == 0) { a.name_off[r] = s0 + 1; a.name_len[r] = e0 - s0 - 1; }
@@ -150,7 +154,7 @@ __global__ void __launch_bounds__(128, 16) k_tok_bases(const TextArgs a) {      
 	const uint32_t lane = threadIdx.x & 31;
 	const uint32_t u = blockIdx.x * 4 + (threadIdx.x >> 5);
 	if(u >= a.n_rec) return;
-	if((*a.tscal & (TX_IRREGULAR | TX_LINECOUNT)) || a.tscal[1] > a.maxlen_hint) return;
+	if((*a.tscal & (TX_IRREGULAR | TX_LINECOUNT)) || a.tscal[3] > a.maxlen_hint) return;
 	uint32_t flags = 0; bool bad = false;
 	const uint64_t total0 = a.off[0][a.n_rec];
 	for(int m = 0; m < a.n_mates; m++) {
@@ -233,7 +237,10 @@ __global__ void __launch_bounds__(128, 16) k_tok_bases(const TextArgs a) {      
 		}
 	}
 	if(__any_sync(0xffffffffu, bad)) { if(lane == 0) atomicOr(a.tscal, (unsigned long long)TX_IRREGULAR); }
-	if(lane == 0) a.flags[u] = (uint8_t)flags;
+	if(lane == 0) {
+		const bool long_unit = !a.keep_long && (a.len[0][u] > kLongUnitLen || (a.n_mates == 2 && a.len[1][u] > kLongUnitLen));
+		a.flags[u] = long_unit ? (uint8_t)0 : (uint8_t)flags;
+	}
 }
 
 // ------------------------------------------------------------------------------ formatter
@@ -260,7 +267,7 @@ struct FmtArgs {
 // A span the tokeniser rejected (or that needs a wider length class) has no valid name / id / flag arrays: the
 // formatter must not touch them.  The bits tested here are final before the formatter starts.
 __device__ __forceinline__ bool span_rejected(const FmtArgs& a) {
-	return (*(volatile unsigned long long*)a.tscal & (TX_IRREGULAR | TX_LINECOUNT)) != 0 || *(volatile unsigned long long*)(a.tscal + 1) > a.maxlen_hint;
+	return (*(volatile unsigned long long*)a.tscal & (TX_IRREGULAR | TX_LINECOUNT)) != 0 || *(volatile unsigned long long*)(a.tscal + 3) > a.maxlen_hint;
 }
 
 __device__ __forceinline__ int find_u64(const uint64_t* a, uint32_t n, uint64_t key) {
@@ -460,7 +467,7 @@ struct TextSlot {
 	DBuf<uint32_t> row_bytes, sec; DBuf<uint64_t> txt_off; DBuf<uint8_t> sel, num;
 	DBuf<char> d_tsv; HBuf<char> h_tsv; DBuf<unsigned long long> multi; HBuf<unsigned long long> h_multi;
 	DBuf<unsigned long long> sp;
-	DBuf<unsigned long long> tscal; HBuf<unsigned long long> h_tscal;    // [0] status [1] maxlen [2] n_multi [3] unused [4],[5] line totals [6] tsv bytes
+	DBuf<unsigned long long> tscal; HBuf<unsigned long long> h_tscal;    // [0] status [1] maxlen [2] n_multi [3] maxlen of mates up to kLongUnitLen [4],[5] line totals [6] tsv bytes
 	uint64_t n_rec = 0; int n_mates = 1; cfb_text_opts opt; uint64_t bytes[2] = {0, 0}; bool pending = false;
 	uint64_t spec_tsv = 0, spec_multi = 0;      // bytes / tie-set records already copied home behind the kernels
 	DBuf<uint8_t> d_cols; std::vector<uint8_t> cols;      // column list of the span in flight (device copy of `cols`)
@@ -607,7 +614,7 @@ static int text_enqueue_all(cfb_ctx* c, Slot& s, TextSlot& t) {
 	}
 	ta.n_rec = (uint32_t)n; ta.lines_per = L; ta.n_mates = nm; ta.fasta = t.opt.fasta ? 1 : 0; ta.trim5 = t.opt.trim5; ta.trim3 = t.opt.trim3; ta.seed = t.opt.seed;
 	ta.flags = s.d_flags.p; ta.name_off = t.name_off.p; ta.name_len = t.name_len.p; ta.id_len = t.id_len.p; ta.bases = s.d_bases.p; ta.tscal = t.tscal.p;
-	ta.maxlen_hint = s.maxlen;
+	ta.maxlen_hint = s.maxlen; ta.keep_long = s.longs.empty() ? 0u : 1u;
 	k_tok_rec<<<(unsigned)((n * nm + 127) / 128), 128, 0, s.st>>>(ta); c->launches++;
 	for(int m = 0; m < nm; m++) {
 		k_scan_sums<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.d_len.p + m * n, n, s.bsum.p);
@@ -643,7 +650,7 @@ extern "C" int cfb_text_submit(cfb_ctx* c, int slot, const void* text_a, uint64_
 	}
 	const int nm = text_b ? 2 : 1; const int L = o->fasta ? 2 : 4;
 	t.n_rec = n_rec; t.n_mates = nm; t.opt = *o; t.bytes[0] = bytes_a; t.bytes[1] = text_b ? bytes_b : 0;
-	s.n_units = n_rec; s.bv.n_units = (uint32_t)n_rec; s.bv.n_mates = nm;
+	s.n_units = n_rec; s.bv.n_units = (uint32_t)n_rec; s.bv.n_mates = nm; s.longs.clear(); s.win_first = 0;
 	if(n_rec == 0) { s.pending = true; t.pending = true; return CFB_OK; }
 	auto pinned = [](const void* p) -> bool {
 		cudaPointerAttributes at;
@@ -693,11 +700,19 @@ extern "C" int cfb_text_wait(cfb_ctx* c, int slot, int discard, cfb_text_result*
 		int rc = finish_batch(c, s, false, false, &r); if(rc) return rc;     // syncs; re-runs classification stages that overflowed
 		const unsigned st = (unsigned)t.h_tscal.p[0];
 		if(st & (TX_IRREGULAR | TX_LINECOUNT)) { out->irregular = 1; return CFB_OK; }
-		const uint32_t maxlen = (uint32_t)t.h_tscal.p[1];
-		out->maxlen = maxlen;
-		if(maxlen > 60000) return fail(CFB_EINVAL, "read longer than 60000 bases");
+		const uint32_t maxlen = (uint32_t)t.h_tscal.p[3];
+		out->maxlen = (uint32_t)t.h_tscal.p[1];
 		if(maxlen > s.maxlen) {          // longer reads than the buffers were sized for: redo the span in a wider class
 			tc.maxlen_hint = std::max(tc.maxlen_hint, len_class(maxlen)); s.maxlen = tc.maxlen_hint;
+			rc = text_enqueue_all(c, s, t); if(rc) return rc;
+			continue;
+		}
+		if(out->maxlen > kLongUnitLen && s.longs.empty()) {     // long records: tokenise again with their flags, and classify them with the long-unit kernels
+			const uint64_t n = t.n_rec; const int nm = t.n_mates;
+			std::vector<uint32_t> lens(n * nm);
+			CK(cudaMemcpy(lens.data(), s.d_len.p, n * nm * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+			const uint32_t* L[2] = {lens.data(), nm == 2 ? lens.data() + n : nullptr};
+			collect_longs(s, n, nm, L, nullptr);
 			rc = text_enqueue_all(c, s, t); if(rc) return rc;
 			continue;
 		}

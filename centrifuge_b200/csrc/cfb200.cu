@@ -556,16 +556,16 @@ struct UnitArgs {
 // twin the CPU tests pin against the oracle) would produce, but reached the way k_search_t reaches them -- K-mer jump, one
 // rank16 entry per step when top and bot share a block, eight bases per walk8 gather of the range's end rows -- so that regenerating
 // a list costs ~30 dependent gathers instead of ~250.  Used by k_prep (lists whose short hits matter) and k_search_long.
-__device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t len, int strand, HitRec* hits, uint32_t cap) {
+// One partial search from `cur` (partial_search_scalar's result) with the device tables.
+__device__ __forceinline__ void partial_search_dev(const IndexView& v, const uint8_t* fw, uint32_t len, int strand, uint32_t cur,
+                                                   HitRec& h, uint32_t& new_cur, bool& done) {
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(v.rank16);
 	const ulonglong2* ftab2 = reinterpret_cast<const ulonglong2*>(v.ftab2);
 	const ulonglong2* ftabk = reinterpret_cast<const ulonglong2*>(v.ftabk);
 	const uint32_t fc = (uint32_t)v.ftab_chars, fk = v.ftabk ? (uint32_t)v.ftabk_chars : 0u;
 	auto base = [&](uint32_t d) -> int { return seq_at(fw, len, strand, len - 1 - d); };     // the base consumed at search depth d
-	uint32_t cur = 0, n = 0;
-	if(len == 0) return 0;
-	for(;;) {
-		HitRec h; h.bwoff = cur; uint32_t new_cur; bool done = false;
+	{
+		h.bwoff = cur; done = false;
 		const uint32_t offset = cur;
 		if(len - cur < fc) { h.top = h.bot = kOff; h.len = len - offset; new_cur = len; done = true; }
 		else {
@@ -610,6 +610,14 @@ __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const
 				}
 			}
 		}
+	}
+}
+__device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t len, int strand, HitRec* hits, uint32_t cap) {
+	uint32_t cur = 0, n = 0;
+	if(len == 0) return 0;
+	for(;;) {
+		HitRec h; uint32_t new_cur; bool done;
+		partial_search_dev(v, fw, len, strand, cur, h, new_cur, done);
 		if(n < cap) hits[n] = h;
 		n++;
 		cur = new_cur;
@@ -995,6 +1003,143 @@ __global__ void __launch_bounds__(128) k_compact(uint32_t n_units, const uint64_
 }
 
 // =======================================================================================
+// Long units (a mate longer than kLongUnitLen bases): segmented search, join and per-unit stages (DESIGN.md section 12a).
+// The batch's other units run the kernels above with the long units' flags cleared; the long units take these kernels,
+// with buffers sized by their own lengths, and share the row buffer, k_lookup and the record scan with them.
+// =======================================================================================
+static const uint32_t kSegLen = 4096;        // bases per speculative chain (DESIGN.md section 12a)
+static_assert(kLongUnitLen == CFB_LONG_UNIT_LEN && kMaxMateLen == CFB_MAX_MATE_LEN, "cf_logic.h and cfb200.h disagree on the read length limits");
+struct LongTask { uint64_t hoff, soff; uint32_t unit, mate, len, nseg; };    // one searched mate: hits at hoff (2 * len slots), segments at soff (2 * nseg)
+struct LongUnit { uint32_t unit, task0, ntask, pad; };
+struct LongArgs {
+	IndexView v; Params p; BatchView b;      // b: the batch's own flags (the short kernels see them with the long units cleared)
+	const LongTask* tasks; uint32_t ntasks; const LongUnit* units; uint32_t nunits; uint64_t nsegs;
+	HitRec* seg; uint32_t* sn; uint32_t* sexit;     // speculative chains
+	HitRec* hits; uint32_t* nh;                     // the true lists, (task, strand) at hits + hoff + strand * len
+	uint32_t* nrows; uint64_t* roff; uint32_t* hl;  // per long unit; hl: EmitRows' whole hit lengths, indexed like the row buffer
+	unsigned long long* stats;                      // [0] speculative partial searches, [1] re-searched at the join
+	UnitArgs u;
+};
+struct DevStep {
+	const IndexView& v; const uint8_t* fw; uint32_t len; int strand; unsigned long long n;
+	__device__ void operator()(uint32_t cur, HitRec& h, uint32_t& nc, bool& done) { partial_search_dev(v, fw, len, strand, cur, h, nc, done); n++; }
+};
+struct ScalarStep {      // CFB_COUNT=1: the scalar search, counting the reference's operations
+	const IndexView& v; const uint8_t* fw; uint32_t len; int strand; Counters* ctr;
+	__device__ void operator()(uint32_t cur, HitRec& h, uint32_t& nc, bool& done) { partial_search_scalar(v, fw, len, strand, cur, h, nc, done, ctr); }
+};
+__device__ __forceinline__ const uint8_t* long_fw(const LongArgs& a, const LongTask& t) { return a.b.bases + (t.mate ? a.b.off[1][t.unit] : a.b.off[0][t.unit]); }
+// the device flags decide which mates count (the text operator's long units are planned before their N filter is known)
+__device__ __forceinline__ bool long_active(const LongArgs& a, const LongTask& t) { return ((a.b.flags[t.unit] >> t.mate) & 1u) != 0; }
+
+// thread per (task, strand, segment): the speculative chain from the segment's first base
+__global__ void __launch_bounds__(128) k_long_seg(const LongArgs a) {
+	const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	unsigned long long n = 0;
+	if(g < a.nsegs) {
+		uint32_t lo = 0, hi = a.ntasks;          // the task holding segment g: the last with soff <= g
+		while(hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if(a.tasks[mid].soff <= g) lo = mid; else hi = mid; }
+		const LongTask t = a.tasks[lo];
+		const uint32_t local = (uint32_t)(g - t.soff), strand = local / t.nseg, k = local - strand * t.nseg;
+		DevStep step{a.v, long_fw(a, t), t.len, (int)strand, 0ull};
+		const uint32_t start = k * kSegLen, stop = min(start + kSegLen, t.len);
+		a.sn[g] = seg_chain(a.p, t.len, start, stop, step, a.seg + t.hoff + (uint64_t)strand * t.len + start, a.sexit + g);
+		n = step.n;
+	}
+	for(int d = 16; d > 0; d >>= 1) n += __shfl_xor_sync(0xffffffffu, n, d);
+	if((threadIdx.x & 31) == 0 && n) atomicAdd(&a.stats[0], n);
+}
+
+// thread per (task, strand): the true chain from the speculative ones.  SCALAR: CFB_COUNT=1, search_strand_scalar itself.
+template <bool SCALAR>
+__global__ void __launch_bounds__(128) k_long_join(const LongArgs a) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= 2 * a.ntasks) return;
+	const LongTask t = a.tasks[i >> 1]; const int strand = (int)(i & 1);
+	HitRec* out = a.hits + t.hoff + (uint64_t)strand * t.len;
+	const uint8_t* fw = long_fw(a, t);
+	if(!long_active(a, t)) { a.nh[i] = 0; return; }
+	if(SCALAR) {
+		Counters local; memset(&local, 0, sizeof local);
+		a.nh[i] = search_strand_scalar(a.v, a.p, fw, t.len, strand, out, t.len, &local);
+		atomicAdd(&a.u.ctr->partial_searches, local.partial_searches); atomicAdd(&a.u.ctr->ftab_probes, local.ftab_probes);
+		atomicAdd(&a.u.ctr->sides_search, local.sides_search); atomicAdd(&a.u.ctr->lf_steps, local.lf_steps);
+		return;
+	}
+	DevStep step{a.v, fw, t.len, strand, 0ull};
+	const uint64_t s0 = t.soff + (uint64_t)strand * t.nseg;
+	unsigned long long re = 0;
+	a.nh[i] = seg_join(a.p, t.len, kSegLen, a.seg + t.hoff + (uint64_t)strand * t.len, a.sn + s0, a.sexit + s0, step, out, &re);
+	if(re) atomicAdd(&a.stats[1], re);
+}
+
+// thread per task: extension, twin removal and trimming of the mate's two lists (post_search_long); the speculative chains'
+// space holds the scratch
+__global__ void __launch_bounds__(128) k_long_post(const LongArgs a) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= a.ntasks) return;
+	const LongTask t = a.tasks[i];
+	Counters local; Counters* lc = nullptr;
+	if(a.u.ctr) { memset(&local, 0, sizeof local); lc = &local; }
+	HitRec* F = a.hits + t.hoff; HitRec* R = F + t.len;
+	post_search_long(a.v, a.p, long_fw(a, t), t.len, F, a.nh[2 * i], R, a.nh[2 * i + 1], reinterpret_cast<uint32_t*>(a.seg + t.hoff), lc);
+	if(lc && local.ext_searches) {
+		atomicAdd(&a.u.ctr->ext_searches, local.ext_searches); atomicAdd(&a.u.ctr->partial_searches, local.partial_searches);
+		atomicAdd(&a.u.ctr->ftab_probes, local.ftab_probes); atomicAdd(&a.u.ctr->sides_search, local.sides_search); atomicAdd(&a.u.ctr->lf_steps, local.lf_steps);
+	}
+}
+
+// thread per long unit: strand choice, sort, row count, a slice of the shared row buffer, rows with the scoring plan (k_prep's
+// work; EMIT_ONLY after the row buffer had to grow)
+template <bool EMIT_ONLY>
+__global__ void __launch_bounds__(32, 1) k_long_prep(const LongArgs a) {      // the register budget of a single warp: the introsort spills below it
+	const uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
+	if(li >= a.nunits) return;
+	const LongUnit lu = a.units[li];
+	UnitHits u; u.n_mates = 0;
+	for(uint32_t k = 0; k < lu.ntask; k++) {
+		const uint32_t ti = lu.task0 + k; const LongTask& t = a.tasks[ti];
+		if(!long_active(a, t)) continue;
+		const int r = u.n_mates++;
+		u.rdlen[r] = t.len;
+		for(int st = 0; st < 2; st++) { u.L[r][st] = a.hits + t.hoff + (uint64_t)st * t.len; u.n[r][st] = a.nh[2 * ti + st]; }
+	}
+	uint64_t rows = 0;
+	if(u.n_mates) {
+		if(EMIT_ONLY) { CountRows cr(a.p, u); for_each_visit(a.p, u, cr); rows = cr.rows; }
+		else { SortAndCount sc(a.p, u); for_each_visit(a.p, u, sc); rows = sc.rows; if(a.u.ctr) atomicAdd(&a.u.ctr->units, 1ull); }
+	}
+	if(rows > 0xFFFFFFFFull) rows = 0xFFFFFFFFull;
+	const uint64_t off = rows ? atomicAdd(a.u.row_total, (unsigned long long)rows) : 0;
+	a.nrows[li] = (uint32_t)rows; a.roff[li] = off;
+	if(rows && off + rows <= a.u.rows_cap) { EmitRows er(a.p, u, a.u.rows + off, a.hl + off); for_each_visit(a.p, u, er); }
+}
+
+// thread per long unit, after k_score: hit map in the global scratch, records into the sparse buffer at the unit's rows, and
+// the unit's record count and row offset for the record scan and k_compact
+__global__ void __launch_bounds__(128) k_long_score(const LongArgs a) {
+	const uint32_t li = blockIdx.x * blockDim.x + threadIdx.x;
+	if(li >= a.nunits || *a.u.row_total > a.u.rows_cap) return;     // else the host grows the row buffer and runs the tail again
+	const LongUnit lu = a.units[li];
+	const uint64_t n = a.nrows[li], off = a.roff[li];
+	uint32_t no = 0;
+	if(n) {
+		Entry* map = a.u.entries + off;
+		const uint32_t nmap = score_plan<true>(a.v, a.p, a.u.rows + off, a.u.ids + off, n, map, a.hl + off);
+		uint32_t mates = 0;
+		for(uint32_t k = 0; k < lu.ntask; k++) mates += long_active(a, a.tasks[lu.task0 + k]) ? 1u : 0u;
+		no = reduce_and_emit(a.v, a.p, mates == 2, map, nmap, a.u.tcs + off, a.u.recs_sparse + off);
+	}
+	a.u.nout[lu.unit] = no; a.u.row_off[lu.unit] = off;
+}
+
+// the short kernels' view of the flags: the long units' cleared
+__global__ void k_mask_long(const LongUnit* units, uint32_t n, uint8_t* flags) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i < n) flags[units[i].unit] = 0;
+}
+
+// =======================================================================================
 // test hook kernels
 // =======================================================================================
 // LF(rows[i], chars[i]) through the scalar LF of cf_logic.h, which reads rank16 on the device; chars[i] > 3 means BWT[rows[i]]
@@ -1295,11 +1440,19 @@ struct Slot {
 	BatchView bv; uint64_t n_units = 0, n_bases = 0; uint32_t maxlen = 0, cap = 0; uint64_t rows_cap = 0, dense_cap = 0;
 	bool pending = false, reran = false;
 	bool want_host = false; uint64_t d2h_recs = 0;     // records already copied to h_recs by the speculative D2H queued behind the kernels
+	// long units of the staged batch (absolute unit index, mate lengths, flags) and the window the kernels run (resident ranges)
+	struct LongH { uint64_t unit; uint32_t len[2]; uint8_t fl; };
+	std::vector<LongH> longs; uint64_t win_first = 0; uint32_t nlong_win = 0;
+	HBuf<LongTask> h_ltask; HBuf<LongUnit> h_lunit; DBuf<LongTask> d_ltask; DBuf<LongUnit> d_lunit;
+	DBuf<HitRec> lseg, lhits; DBuf<uint32_t> lsn, lsexit, lnh, lnrows, lhl; DBuf<uint64_t> lroff; DBuf<uint8_t> flags_short; DBuf<unsigned long long> lstats;
+	uint64_t lhit_slots = 0, lsegs = 0; uint32_t lntasks = 0, lmaxlen = 0;
 	void release() {
 		h_bases.release(); h_off.release(); h_len.release(); h_flags.release(); d_bases.release(); d_off.release(); d_len.release(); d_flags.release();
 		h_words.release(); d_words.release(); d_npos.release(); d_woff.release(); d_wlen.release();
 		pk.release(); nm.release(); hits.release(); nhits.release(); regen.release(); regen_n.release(); nrows.release(); row_off.release(); bsum.release(); rows.release(); ids.release(); entries.release(); tcs.release();
 		sparse.release(); nout.release(); out_off.release(); scan_tmp.release(); dense.release(); rec_off32.release(); scal.release(); h_scal.release(); h_recs.release(); h_rec_off.release(); cnt.release();
+		h_ltask.release(); h_lunit.release(); d_ltask.release(); d_lunit.release(); lseg.release(); lhits.release(); lsn.release(); lsexit.release(); lnh.release();
+		lnrows.release(); lhl.release(); lroff.release(); flags_short.release(); lstats.release();
 		for(int i = 0; i < 6; i++) if(ev[i]) cudaEventDestroy(ev[i]);
 		if(st) cudaStreamDestroy(st);
 	}
@@ -1336,6 +1489,7 @@ struct cfb_ctx {
 	TextCtx* text = nullptr;
 	CountsCtx cnt; bool fold_records = false;
 	bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
+	uint64_t long_units = 0, long_bases = 0, long_searches = 0, long_researched = 0;    // cfb_ctx_long_stats
 	uint64_t regen_lists = 0, regen_tasks = 0;   // lists regenerated / strand lists searched so far (CFB_REGEN_STATS=1 prints them when the context goes)
 	uint64_t regen_slots0 = 0;    // CFB_REGEN_SLOTS: initial capacity of the list-regeneration buffer (tests force the grow-and-re-run path with it)
 	void* comm = nullptr; int comm_rank = 0, comm_size = 1; cudaStream_t comm_st = nullptr;      // NCCL communicator (cf_multi.cuh)
@@ -1512,6 +1666,34 @@ __global__ void k_cnt_commit(const unsigned long long* slot_sp, unsigned long lo
 }
 
 // Validate + stage a batch into the slot's pinned buffers and enqueue H2D copies.
+// Device memory a batch with long units could not get: CFB_ENOMEM naming the long reads (other batches report CFB_ECUDA as before)
+static int long_oom(const Slot& s, cudaError_t e, const char* what) {
+	cudaGetLastError();
+	uint64_t bases = 0; uint32_t mx = 0;
+	for(const Slot::LongH& l : s.longs) { bases += (uint64_t)l.len[0] + l.len[1]; mx = std::max(mx, std::max(l.len[0], l.len[1])); }
+	return fail(CFB_ENOMEM, "no device memory for %s of a batch with %zu long units (%llu bases, the longest read %u bases): %s", what,
+	            s.longs.size(), (unsigned long long)bases, mx, cudaGetErrorString(e));
+}
+// CK for buffers whose size long units drive
+#define CKL(call, what) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { if(!s.longs.empty()) return long_oom(s, e_, what); CK(e_); } } while(0)
+
+static int mate_too_long(uint64_t n, int m, const uint32_t* L) {
+	for(uint64_t i = 0; i < n; i++)
+		if(L[i] > kMaxMateLen) return fail(CFB_EINVAL, "unit %llu mate %d has %u bases: the limit is %u bases per mate", (unsigned long long)i, m + 1, L[i], kMaxMateLen);
+	return CFB_OK;
+}
+// Units with a mate longer than kLongUnitLen go to the long-unit kernels (their flags are cleared for the others).  Returns the
+// longest mate of the remaining units, which sizes the short kernels' buffers as before.
+static uint32_t collect_longs(Slot& s, uint64_t n, int nm, const uint32_t* const len[2], const uint8_t* flags) {
+	uint32_t mx = 0;
+	for(uint64_t i = 0; i < n; i++) {
+		const uint32_t l0 = len[0][i], l1 = nm == 2 ? len[1][i] : 0;
+		if(l0 > kLongUnitLen || l1 > kLongUnitLen) s.longs.push_back(Slot::LongH{i, {l0, l1}, flags ? flags[i] : (uint8_t)3});
+		else mx = std::max(mx, std::max(l0, l1));
+	}
+	return mx;
+}
+
 static int stage_batch(cfb_ctx* c, Slot& s, const cfb_batch* b) {
 	if(!b || b->n_mates < 1 || b->n_mates > 2 || !b->bases || !b->off[0] || !b->len[0] || (b->n_mates == 2 && (!b->off[1] || !b->len[1])))
 		return fail(CFB_EINVAL, "malformed cfb_batch");
@@ -1521,12 +1703,14 @@ static int stage_batch(cfb_ctx* c, Slot& s, const cfb_batch* b) {
 	for(int m = 0; m < nm; m++) {       // branch-free validation pass (vectorises); the offender is looked up only when there is one
 		const uint64_t* O = b->off[m]; const uint32_t* L = b->len[m]; const uint64_t nb = b->n_bases; uint32_t mx = 0; uint64_t far = 0;
 		for(uint64_t i = 0; i < n; i++) { const uint32_t l = L[i]; mx = l > mx ? l : mx; }
+		if(mx > kMaxMateLen) return mate_too_long(n, m, L);
 		for(uint64_t i = 0; i < n; i++) { const uint64_t e = O[i] + (uint64_t)L[i]; far = e > far ? e : far; }
 		if(far > nb) { for(uint64_t i = 0; i < n; i++) if(O[i] + L[i] > nb) return fail(CFB_EINVAL, "unit %llu mate %d exceeds n_bases", (unsigned long long)i, m + 1); }
 		maxlen = std::max(maxlen, mx);
 	}
-	if(maxlen > 60000) return fail(CFB_EINVAL, "read longer than 60000 bases");
-	CK(s.d_bases.ensure(b->n_bases + 16)); CK(s.d_off.ensure(n * nm)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
+	s.longs.clear(); s.win_first = 0;
+	if(maxlen > kLongUnitLen) maxlen = collect_longs(s, n, nm, b->len, b->flags);
+	CKL(s.d_bases.ensure(b->n_bases + 16), "the bases"); CK(s.d_off.ensure(n * nm)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
 	// Caller arrays that already live in pinned memory (cfb_host_alloc) are DMA'd from where they are and
 	// must stay untouched until cfb_classify_wait; pageable arrays are staged through pinned buffers first.
 	auto pinned = [](const void* p) -> bool {
@@ -1600,11 +1784,13 @@ static int stage_batch_packed(cfb_ctx* c, Slot& s, const cfb_batch_packed* b) {
 		for(uint64_t i = 0; i < n; i++) { const uint32_t l = L[i]; mx = l > mx ? l : mx; w += (l + 31u) >> 5; }
 		maxlen = std::max(maxlen, mx); mate_words[m] = w; need_words += w;
 	}
+	for(int m = 0; m < nm; m++) { const int rc = mate_too_long(n, m, b->len[m]); if(rc) return rc; }
 	if(need_words != b->n_words) return fail(CFB_EINVAL, "cfb_batch_packed: n_words is %llu, the lengths need %llu", (unsigned long long)b->n_words, (unsigned long long)need_words);
-	if(maxlen > 60000) return fail(CFB_EINVAL, "read longer than 60000 bases");
+	s.longs.clear(); s.win_first = 0;
+	if(maxlen > kLongUnitLen) maxlen = collect_longs(s, n, nm, b->len, b->flags);
 	const uint64_t scan_blocks = (n + kScanBlock * kScanPer - 1) / (kScanBlock * kScanPer);
-	CK(s.d_bases.ensure(b->n_words * 32 + 64)); CK(s.d_off.ensure(n * nm + 1)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
-	CK(s.d_words.ensure(b->n_words + 1)); CK(s.d_npos.ensure(b->n_n + 1)); CK(s.d_wlen.ensure(n + 1)); CK(s.d_woff.ensure(n + 2)); CK(s.bsum.ensure(scan_blocks + 1));
+	CKL(s.d_bases.ensure(b->n_words * 32 + 64), "the bases"); CK(s.d_off.ensure(n * nm + 1)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
+	CKL(s.d_words.ensure(b->n_words + 1), "the packed bases"); CK(s.d_npos.ensure(b->n_n + 1)); CK(s.d_wlen.ensure(n + 1)); CK(s.d_woff.ensure(n + 2)); CK(s.bsum.ensure(scan_blocks + 1));
 	auto pinned = [](const void* p) -> bool {
 		cudaPointerAttributes at;
 		if(cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
@@ -1637,6 +1823,12 @@ static int stage_batch_packed(cfb_ctx* c, Slot& s, const cfb_batch_packed* b) {
 		k_scan_apply<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.d_wlen.p, n, s.bsum.p, (const uint64_t*)(s.scal.p + 5), s.d_woff.p);
 		if(W) k_unpack<<<(unsigned)((n * W + 255) / 256), 256, 0, s.st>>>(s.d_words.p, s.d_woff.p, wbase, s.d_len.p + m * n, n, W, s.d_bases.p, s.d_off.p + m * n);
 		c->launches += 5;
+		for(const Slot::LongH& l : s.longs) {      // W covers the other units: a long mate is expanded by a launch of its own
+			const uint32_t Wl = (l.len[m] + 31) / 32;
+			if(Wl <= W) continue;
+			k_unpack<<<(unsigned)((Wl + 255) / 256), 256, 0, s.st>>>(s.d_words.p, s.d_woff.p + l.unit, wbase, s.d_len.p + m * n + l.unit, 1, Wl, s.d_bases.p, s.d_off.p + m * n + l.unit);
+			c->launches++;
+		}
 		wbase += mate_words[m];      // mate 2 starts after all of mate 1
 	}
 	if(b->n_n) { k_set_n<<<(unsigned)((b->n_n + 255) / 256), 256, 0, s.st>>>(s.d_npos.p, b->n_n, s.d_bases.p, b->n_words * 32); c->launches++; }
@@ -1647,11 +1839,56 @@ static int stage_batch_packed(cfb_ctx* c, Slot& s, const cfb_batch_packed* b) {
 	return CFB_OK;
 }
 
+// The long units of the slot's window [win_first, win_first + n_units): their searched mates (tasks), with hit and segment
+// space laid out by prefix sums over their own lengths, uploaded for the long-unit kernels.
+static int long_plan(cfb_ctx* c, Slot& s) {
+	s.nlong_win = 0; s.lntasks = 0; s.lhit_slots = 0; s.lsegs = 0; s.lmaxlen = 0;
+	if(s.longs.empty()) return CFB_OK;
+	const uint64_t lo = s.win_first, hi = s.win_first + s.n_units;
+	CK(s.h_lunit.ensure(s.longs.size())); CK(s.h_ltask.ensure(2 * s.longs.size()));
+	uint32_t nu = 0, nt = 0;
+	for(const Slot::LongH& l : s.longs) {
+		if(l.unit < lo || l.unit >= hi) continue;
+		LongUnit u; u.unit = (uint32_t)(l.unit - lo); u.task0 = nt; u.ntask = 0; u.pad = 0;
+		for(int m = 0; m < s.bv.n_mates; m++) {
+			if(!((l.fl >> m) & 1) || l.len[m] == 0) continue;
+			LongTask t; t.hoff = s.lhit_slots; t.soff = s.lsegs; t.unit = u.unit; t.mate = (uint32_t)m; t.len = l.len[m];
+			t.nseg = (t.len + kSegLen - 1) / kSegLen;
+			s.lhit_slots += 2ull * t.len; s.lsegs += 2ull * t.nseg; s.lmaxlen = std::max(s.lmaxlen, t.len);
+			s.h_ltask.p[nt++] = t; u.ntask++;
+		}
+		s.h_lunit.p[nu++] = u;
+	}
+	s.nlong_win = nu; s.lntasks = nt;
+	if(nu == 0) return CFB_OK;
+	auto grow = [&](cudaError_t e) -> int {
+		if(e == cudaSuccess) return CFB_OK;
+		cudaGetLastError();
+		return fail(CFB_ENOMEM, "no device memory for the long reads of this batch: %llu bases in %u long mates, the longest %u bases",
+		            (unsigned long long)(s.lhit_slots / 2), nt, s.lmaxlen);
+	};
+	int rc;
+	if((rc = grow(s.d_lunit.ensure(nu))) || (rc = grow(s.d_ltask.ensure(nt + 1))) || (rc = grow(s.lseg.ensure(s.lhit_slots + 1))) ||
+	   (rc = grow(s.lhits.ensure(s.lhit_slots + 1))) || (rc = grow(s.lsn.ensure(s.lsegs + 1))) || (rc = grow(s.lsexit.ensure(s.lsegs + 1))) ||
+	   (rc = grow(s.lnh.ensure(2ull * nt + 1))) || (rc = grow(s.lnrows.ensure(nu))) || (rc = grow(s.lroff.ensure(nu))) ||
+	   (rc = grow(s.flags_short.ensure(s.n_units))) || (rc = grow(s.lstats.ensure(2)))) return rc;
+	CK(cudaMemcpyAsync(s.d_lunit.p, s.h_lunit.p, nu * sizeof(LongUnit), cudaMemcpyHostToDevice, s.st));
+	CK(cudaMemcpyAsync(s.d_ltask.p, s.h_ltask.p, nt * sizeof(LongTask), cudaMemcpyHostToDevice, s.st));
+	CK(cudaMemsetAsync(s.lnh.p, 0, (2ull * nt + 1) * sizeof(uint32_t), s.st));
+	CK(cudaMemsetAsync(s.lstats.p, 0, 2 * sizeof(unsigned long long), s.st));
+	CK(cudaMemcpyAsync(s.flags_short.p, s.bv.flags, s.n_units, cudaMemcpyDeviceToDevice, s.st));
+	k_mask_long<<<(nu + 127) / 128, 128, 0, s.st>>>(s.d_lunit.p, nu, s.flags_short.p); c->launches++;
+	return CFB_OK;
+}
+
 // Enqueue all kernels of one batch on the slot's stream.  stage: 0 = from search, 1 = from k_rows
 // (after a rows-capacity overflow; the hit lists are already post-processed and sorted).
 static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	const uint64_t n = s.n_units; const int nm = s.bv.n_mates;
 	const uint64_t ntasks = n * nm * 2;
+	if(stage == 0 && n) { const int rc = long_plan(c, s); if(rc) return rc; }
+	BatchView sb = s.bv;                 // what the short kernels see: the long units' flags cleared
+	if(s.nlong_win) sb.flags = s.flags_short.p;
 	const uint32_t ublocks = (uint32_t)((n + 127) / 128);
 	const uint64_t scan_blocks = (n + kScanBlock * kScanPer - 1) / (kScanBlock * kScanPer);
 	if(n == 0) return CFB_OK;
@@ -1676,6 +1913,11 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 		CK(s.bsum.ensure(scan_blocks + 1)); CK(s.nout.ensure(n + 1)); CK(s.out_off.ensure(n + 1)); CK(s.rec_off32.ensure(n + 1));
 		s.rows_cap = std::max<uint64_t>(s.rows_cap, c->rows_cap0 ? c->rows_cap0 : std::max<uint64_t>(n * 12, 4096));
 	}
+	if(s.nlong_win) {
+		CKL(s.rows.ensure(s.rows_cap), "the rows"); CKL(s.ids.ensure(s.rows_cap), "the rows"); CKL(s.entries.ensure(s.rows_cap), "the hit maps");
+		CKL(s.tcs.ensure(s.rows_cap), "the hit maps"); CKL(s.sparse.ensure(s.rows_cap), "the records"); CKL(s.dense.ensure(s.rows_cap), "the records");
+		CKL(s.lhl.ensure(s.rows_cap), "the rows");
+	}
 	CK(s.rows.ensure(s.rows_cap)); CK(s.ids.ensure(s.rows_cap)); CK(s.entries.ensure(s.rows_cap)); CK(s.tcs.ensure(s.rows_cap)); CK(s.sparse.ensure(s.rows_cap));
 	s.dense_cap = s.rows_cap; CK(s.dense.ensure(s.dense_cap));
 	CK(cudaMemsetAsync(s.scal.p, 0, 4 * sizeof(unsigned long long), s.st));   // task counters, overflow flag, row allocator; [4] is rewritten by the scan
@@ -1686,16 +1928,16 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 		const size_t sc0 = offsetof(Counters, sc_units);
 		CK(cudaMemsetAsync(reinterpret_cast<char*>(c->d_ctr) + sc0, 0, sizeof(Counters) - sc0, s.st));
 	}
-	UnitArgs ua; ua.v = c->view; ua.p = c->prm; ua.b = s.bv; ua.hits = s.hits.p; ua.nhits = s.nhits.p; ua.cap = s.cap;
+	UnitArgs ua; ua.v = c->view; ua.p = c->prm; ua.b = sb; ua.hits = s.hits.p; ua.nhits = s.nhits.p; ua.cap = s.cap;
 	ua.nrows = s.nrows.p; ua.row_off = s.row_off.p; ua.row_total = s.scal.p + 3; ua.rows = s.rows.p; ua.ids = s.ids.p; ua.rows_cap = s.rows_cap;
 	ua.entries = s.entries.p; ua.tcs = s.tcs.p; ua.recs_sparse = s.sparse.p; ua.nout = s.nout.p;
 	ua.overflow = (unsigned int*)(s.scal.p + 2); ua.ctr = ctr;
 	ua.regen = s.regen.p; ua.regen_n = s.regen_n.p; ua.regen_ctr = s.scal.p + 6; ua.regen_slots = s.regen_slots; ua.full_cap = s.full_cap; ua.keep_short = keep_short ? 1u : 0u;
 	if(stage == 0) {
-		SearchArgs sa; sa.v = c->view; sa.p = c->prm; sa.b = s.bv; sa.hits = s.hits.p; sa.nhits = s.nhits.p; sa.cap = s.cap;
+		SearchArgs sa; sa.v = c->view; sa.p = c->prm; sa.b = sb; sa.hits = s.hits.p; sa.nhits = s.nhits.p; sa.cap = s.cap;
 		const uint32_t W = (s.maxlen + 31) / 32 + 1;
 		sa.pk = s.pk.p; sa.nm = s.nm.p; sa.W = W; sa.keep_short = keep_short ? 1u : 0u;
-		{ PackArgs pa; pa.b = s.bv; pa.pk = s.pk.p; pa.nm = s.nm.p; pa.W = W;
+		{ PackArgs pa; pa.b = sb; pa.pk = s.pk.p; pa.nm = s.nm.p; pa.W = W;
 		  k_pack<<<(unsigned)((ntasks * W + 127) / 128), 128, 0, s.st>>>(pa); c->launches++; }
 		sa.task_ctr64 = s.scal.p + 0; sa.ntasks = (uint32_t)ntasks; sa.overflow = (unsigned int*)(s.scal.p + 2); sa.ctr = ctr;
 		int occ = 1;
@@ -1712,6 +1954,26 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 		if(time_it) CK(cudaEventRecord(s.ev[1], s.st));
 		k_prep<8, true><<<ublocks, 128, 0, s.st>>>(ua); c->launches++;
 	}
+	LongArgs la;
+	if(s.nlong_win) {
+		la.v = c->view; la.p = c->prm; la.b = s.bv; la.tasks = s.d_ltask.p; la.ntasks = s.lntasks; la.units = s.d_lunit.p; la.nunits = s.nlong_win;
+		la.nsegs = s.lsegs; la.seg = s.lseg.p; la.sn = s.lsn.p; la.sexit = s.lsexit.p; la.hits = s.lhits.p; la.nh = s.lnh.p;
+		la.nrows = s.lnrows.p; la.roff = s.lroff.p; la.hl = s.lhl.p; la.stats = s.lstats.p; la.u = ua;
+		const unsigned ub = (s.nlong_win + 31) / 32;
+		if(stage == 0) {
+			if(s.lntasks) {
+				if(c->count == 1) k_long_join<true><<<(2 * s.lntasks + 127) / 128, 128, 0, s.st>>>(la);
+				else {
+					k_long_seg<<<(unsigned)((s.lsegs + 127) / 128), 128, 0, s.st>>>(la);
+					k_long_join<false><<<(2 * s.lntasks + 127) / 128, 128, 0, s.st>>>(la);
+				}
+				k_long_post<<<(s.lntasks + 127) / 128, 128, 0, s.st>>>(la);
+				c->launches += c->count == 1 ? 2 : 3;
+			}
+			k_long_prep<false><<<ub, 32, 0, s.st>>>(la);
+		} else k_long_prep<true><<<ub, 32, 0, s.st>>>(la);
+		c->launches++;
+	}
 	if(time_it) CK(cudaEventRecord(s.ev[2], s.st));
 	ResolveArgs ra; ra.v = c->view; ra.rows = s.rows.p; ra.ids = s.ids.p; ra.ids16 = nullptr; ra.total = (const uint64_t*)(s.scal.p + 3); ra.rows_cap = s.rows_cap;
 	ra.task_ctr = s.scal.p + 1; ra.chunk = 64; ra.ctr = ctr;
@@ -1722,6 +1984,7 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	if(time_it) CK(cudaEventRecord(s.ev[3], s.st));
 	if(ctr) k_score<12, true><<<ublocks, kScoreThreads, 0, s.st>>>(ua);
 	else k_score<12, false><<<ublocks, kScoreThreads, 0, s.st>>>(ua);        // <= 40 registers and 14.5 KB of shared memory: 12 CTAs per SM
+	if(s.nlong_win) { k_long_score<<<(s.nlong_win + 127) / 128, 128, 0, s.st>>>(la); c->launches++; }
 	// record offsets: one single-pass scan over the n + 1 counts (the last is 0, so out_off[n] is the total), in 64 bits
 	size_t scan_bytes = 0;
 	CK(cub::DeviceScan::ExclusiveScan(nullptr, scan_bytes, s.nout.p, s.out_off.p, cub::Sum(), (uint64_t)0, (int)(n + 1), s.st));
@@ -1783,6 +2046,11 @@ static int finish_batch(cfb_ctx* c, Slot& s, bool time_it, bool to_host, cfb_res
 	}
 	const uint64_t nrec = s.h_scal.p[4];
 	c->regen_lists += s.h_scal.p[6]; c->regen_tasks += (uint64_t)s.n_units * (uint64_t)s.bv.n_mates * 2;
+	if(s.nlong_win) {
+		unsigned long long st[2];
+		CK(cudaMemcpy(st, s.lstats.p, sizeof st, cudaMemcpyDeviceToHost));
+		c->long_units += s.nlong_win; c->long_bases += s.lhit_slots / 2; c->long_searches += st[0]; c->long_researched += st[1];
+	}
 	if(s.folded) {        // the batch is final: add its counters to the context's totals (stream order keeps this ahead of any read)
 		const uint32_t n3 = 3 * c->cnt.n;
 		k_cnt_commit<<<(n3 + 255) / 256, 256, 0, s.st>>>(s.cnt.p, c->cnt.total.p, n3); c->launches++;
@@ -1884,7 +2152,7 @@ extern "C" int cfb_classify_resident_range(cfb_ctx* c, cfb_dbatch* d, uint64_t f
 	Slot& s = c->slots[d->slot];
 	// a window of the uploaded batch: offsets are absolute into the uploaded bases, so only the per-unit arrays shift
 	const uint64_t N = d->n_units; const int nmates = s.bv.n_mates;
-	s.bv.flags = s.d_flags.p + first; s.bv.n_units = (uint32_t)count; s.n_units = count;
+	s.bv.flags = s.d_flags.p + first; s.bv.n_units = (uint32_t)count; s.n_units = count; s.win_first = first;
 	for(int m = 0; m < nmates; m++) { s.bv.off[m] = s.d_off.p + m * N + first; s.bv.len[m] = s.d_len.p + m * N + first; }
 	int rc = enqueue_kernels(c, s, 0, true); if(rc) return rc;
 	cfb_result r;
@@ -1903,6 +2171,11 @@ extern "C" int cfb_resident_result(cfb_ctx* c, cfb_result* out) {
 	CK(cudaSetDevice(c->ix->device));
 	Slot& s = c->slots[kSlots - 1];
 	return finish_batch(c, s, false, true, out);
+}
+extern "C" int cfb_ctx_long_stats(const cfb_ctx* c, uint64_t out[4]) {
+	if(!c || !out) return fail(CFB_EINVAL, "null argument");
+	out[0] = c->long_units; out[1] = c->long_bases; out[2] = c->long_searches; out[3] = c->long_researched;
+	return CFB_OK;
 }
 extern "C" int cfb_ctx_counters(cfb_ctx* c, uint64_t out[8]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");

@@ -122,6 +122,13 @@ typedef struct {
 	const uint32_t* len[2];
 	const uint8_t*  flags;       /* NULL = all mates pass */
 } cfb_batch;
+/* Read length.  A mate may hold up to CFB_MAX_MATE_LEN bases (2^31 - 1, so that len1 + len2 and cfb_rec.hitlen stay in 32
+ * bits); a longer one makes every classify entry point return CFB_EINVAL.  A unit with a mate longer than CFB_LONG_UNIT_LEN
+ * bases (a long unit) is searched in parallel segments by kernels of its own, with device memory sized by its own length
+ * (about 100 bytes per base of its mates); its records come back in unit order with the others.  When that memory cannot be
+ * had the batch fails with CFB_ENOMEM and cfb_last_error() names the lengths. */
+#define CFB_MAX_MATE_LEN  2147483647u
+#define CFB_LONG_UNIT_LEN 60000u
 
 /* One AlnRes worth of data (aligner_result.h:321): what Classifier::go hands sink.report(). */
 typedef struct {
@@ -283,6 +290,9 @@ int cfb_ctx_score_stats(cfb_ctx*, uint64_t out[23]);
  * table-free restatement of the reference's walk (same definition as SURVEY.md 8d):
  * {units, partial_searches, ftab_probes, sides_search, walk_steps, rows_resolved, lf_steps_total, ext_searches} */
 int cfb_ctx_counters(cfb_ctx*, uint64_t out[8]);
+/* Long units classified by this ctx so far: {long units, bases of their searched mates, partial searches of the speculative
+ * segment chains, partial searches the join ran again}. */
+int cfb_ctx_long_stats(const cfb_ctx*, uint64_t out[4]);
 int cfb_ctx_kernel_launches(const cfb_ctx*, uint64_t* n);
 
 int   cfb_device_count(void);         /* usable CUDA devices (0 without a driver) */
