@@ -1615,7 +1615,9 @@ extern "C" int cfb_run(int argc, const char** argv) {
 		}
 		if(getenv("CFB_TEXT_STATS")) {
 			const auto t_done = std::chrono::steady_clock::now();
-			std::cerr << "[cfb] index load " << std::chrono::duration<double>(t_loaded - t_start).count() << " s, reads " << std::chrono::duration<double>(t_done - t_loaded).count() << " s" << std::endl;
+			cfb_index_tables tb; memset(&tb, 0, sizeof tb); cfb_index_get_tables(rs.ix[0], &tb);
+			std::cerr << "[cfb] index load " << std::chrono::duration<double>(t_loaded - t_start).count() << " s (" << (tb.rank16_bytes ? "rank16" : "compact")
+			          << " rank layout), reads " << std::chrono::duration<double>(t_done - t_loaded).count() << " s" << std::endl;
 			std::cerr << "[cfb] text operator: " << tstats.units << " units in " << tstats.spans << " spans (" << tstats.bytes_in << " bytes in, " << tstats.bytes_out
 			          << " bytes out, " << tstats.fallbacks << " fallbacks); record-level reader: " << host_units << " units" << std::endl;
 			uint64_t lt[4] = {0, 0, 0, 0};

@@ -60,6 +60,8 @@ struct IndexView {
 	const uint16_t* rtab16;         // device-only resolve table: sequence id of EVERY SA row (one of rtab16/rtab32, or neither)
 	const uint32_t* rtab32;
 	const uint64_t* ftabk;          // device-only K-mer jump table: (top | width << 40, death bitmap) per K-mer, K = ftabk_chars, see k_build_ftabk (null = absent)
+	const uint64_t* cr;             // device-only compact rank layout (when rank16 does not fit): 64-byte half-sides, format and decoders below (null = absent)
+	const uint64_t* crsb;           // its superblock table: occ of every base before each superblock's first half-side, 4 x u64 per superblock
 	const uint64_t* walk8;          // device-only: per SA row, the row 8 LF steps on | the 8 BWT bases met << 40 | #valid steps << 56 (null = absent)
 	uint64_t walk8_rows;            // rows [0, walk8_rows) have a walk8 entry (the table may cover a prefix of the rows when HBM is short)
 	int32_t  ftabd_chars;           // K + 3 while the K-mer table carries the death bitmap, else 0
@@ -161,6 +163,97 @@ CFB_HD uint64_t match2(uint64_t w, int c) {
 	return y & (y >> 1) & 0x5555555555555555ull;
 }
 
+// Compact rank layout (IndexView::cr, 1/3 byte per row): half-side h covers rows [192h, 192h + 192) in 64 bytes:
+//   u32 cnt[4] (occ of c before the half-side, '$' excluded, minus the superblock's entry)  |  6 x u64 of 2-bit BWT, 32 rows each
+// The '$' row is stored as A and corrected for (the zOff rule of countBt2Side, bt2_idx.h:2192-2227); padding after the last row
+// reads as A.  Side i of the .1.cf file becomes half-sides 2i and 2i+1 in the same 128 bytes (cr_convert_side), so the layout is
+// built in place from the streamed sides.  A superblock is 2^SB half-sides; crsb holds the absolute occ before its first
+// half-side.  A rank query reads the count piece and the words before its offset: one 32-byte sector for offsets up to 64, two
+// beyond.  SB >= 1 (a superblock starts on a side) and 192 << SB < 2^32 (the relative counts fit their 32 bits).
+static const uint32_t kCrRows = 192;
+static const int kCrSbShift = 24;           // 2^24 half-sides = 3.2 G rows per superblock
+template <int SB> struct CrSbCheck { static_assert(SB >= 1 && (192ull << SB) < (1ull << 32), "superblock span out of range"); };
+// number of half-sides including the sentinel one past the last side (an exclusive bound len + 1 on a side boundary reads it)
+CFB_HD uint64_t cr_halves(uint64_t num_sides) { return 2 * num_sides + 1; }
+template <int SB = kCrSbShift> CFB_HD uint64_t cr_superblocks(uint64_t num_sides) { return (cr_halves(num_sides) + (1ull << SB) - 1) >> SB; }
+// occ of c in the 2-bit words w[0, nw) ('$' at position zpos counted out when zpos < 32 * nw)
+CFB_HD void cr_count_words(const uint64_t* w, int nw, uint64_t zpos, uint64_t occ[4]) {
+	for(int k = 0; k < nw; k++) for(int c = 0; c < 4; c++) occ[c] += (uint64_t)popc64(match2(w[k], c));
+	if(zpos < (uint64_t)nw * 32) occ[0] -= 1;
+}
+// crsb entry of superblock sb, read from the file's sides before they are converted
+template <int SB = kCrSbShift> CFB_HD void cr_sb_entry(const uint64_t* sides, uint64_t num_sides, uint64_t zoff, uint64_t sb, uint64_t* out) {
+	(void)CrSbCheck<SB>();
+	const uint64_t s = sb << (SB - 1);
+	if(s < num_sides) { for(int c = 0; c < 4; c++) out[c] = sides[s * 16 + 12 + c]; return; }
+	const uint64_t* w = sides + (num_sides - 1) * 16;        // the sentinel half-side's superblock: the totals
+	uint64_t occ[4] = {w[12], w[13], w[14], w[15]};
+	cr_count_words(w, 12, zoff - (num_sides - 1) * 384, occ);
+	for(int c = 0; c < 4; c++) out[c] = occ[c];
+}
+// Side i -> half-sides 2i, 2i+1 in place (the last side also writes the sentinel half-side into the 64 bytes after it).  Reads
+// the whole side before it writes, so one thread per side needs no second copy.  sb: the finished superblock table.
+template <int SB = kCrSbShift> CFB_HD void cr_convert_side(uint64_t* sides, uint64_t num_sides, uint64_t zoff, const uint64_t* sb, uint64_t i) {
+	(void)CrSbCheck<SB>();
+	uint64_t w[16];
+	for(int k = 0; k < 16; k++) w[k] = sides[i * 16 + k];
+	uint64_t occ[4] = {w[12], w[13], w[14], w[15]};
+	const uint64_t zpos = zoff - i * 384;      // wraps to a huge value when '$' lies before the side
+	uint64_t* out = sides + i * 16;
+	const int nh = i + 1 == num_sides ? 3 : 2;
+	for(int k = 0; k < nh; k++) {
+		const uint64_t h = 2 * i + (uint64_t)k, base = (h >> SB) * 4;
+		out[k * 8] = (occ[0] - sb[base]) | ((occ[1] - sb[base + 1]) << 32);
+		out[k * 8 + 1] = (occ[2] - sb[base + 2]) | ((occ[3] - sb[base + 3]) << 32);
+		for(int j = 0; j < 6; j++) out[k * 8 + 2 + j] = k < 2 ? w[k * 6 + j] : 0ull;
+		if(k < 2) cr_count_words(w + k * 6, 6, zpos - (uint64_t)k * 192, occ);
+	}
+}
+// LF(row, c) and BWT[row] on the compact layout.  The device reads the second sector only when the offset needs it.
+template <int SB = kCrSbShift> CFB_HD uint64_t cr_lf(const IndexView& v, uint64_t row, int c) {
+	const uint64_t h = row / kCrRows; const uint32_t o = (uint32_t)(row - h * kCrRows);
+	const uint64_t* p = v.cr + h * 8;
+	uint64_t q[8];
+#ifdef __CUDA_ARCH__
+	const ulonglong2 a = __ldg(reinterpret_cast<const ulonglong2*>(p)), b = __ldg(reinterpret_cast<const ulonglong2*>(p) + 1);
+	q[0] = a.x; q[1] = a.y; q[2] = b.x; q[3] = b.y; q[4] = q[5] = q[6] = q[7] = 0;
+	if(o > 64) {
+		const ulonglong2 d = __ldg(reinterpret_cast<const ulonglong2*>(p) + 2), e = __ldg(reinterpret_cast<const ulonglong2*>(p) + 3);
+		q[4] = d.x; q[5] = d.y; q[6] = e.x; q[7] = e.y;
+	}
+#else
+	for(int k = 0; k < 8; k++) q[k] = p[k];
+#endif
+	const uint32_t full = o >> 5, rem = o & 31;
+	uint64_t n = ((c < 2 ? q[0] : q[1]) >> (32 * (c & 1))) & 0xffffffffull;
+#ifdef __CUDA_ARCH__
+	#pragma unroll
+#endif
+	for(uint32_t k = 0; k < 6; k++) {
+		const uint64_t m = k < full ? ~0ull : (k == full ? (((uint64_t)1 << (2 * rem)) - 1) : 0ull);
+		n += (uint64_t)popc64(match2(q[2 + k], c) & m);
+	}
+	if(c == 0 && v.zoff < row && v.zoff >= row - o) n--;
+	return v.fchr[c] + v.crsb[(h >> SB) * 4 + (uint64_t)c] + n;
+}
+CFB_HD int cr_bwt(const IndexView& v, uint64_t row) {
+	const uint64_t h = row / kCrRows; const uint32_t o = (uint32_t)(row - h * kCrRows);
+	return (int)((v.cr[h * 8 + 2 + (o >> 5)] >> ((o & 31) * 2)) & 3);
+}
+
+// Which rank layout a replica loads (cfb_index_load_ex), decided from free device memory before anything is allocated:
+// rank16 when the transient sides, rank16, the sample, the fixed tables and the head-room all fit; else the compact layout when
+// it, the sample, the fixed tables and the head-room fit; else none (-1).  force_compact skips rank16.
+enum { kLayoutNone = -1, kLayoutRank16 = 0, kLayoutCompact = 1 };
+CFB_HD uint64_t rank16_bytes_for(uint64_t num_sides) { return (num_sides * 6 + 1) * 64; }
+CFB_HD uint64_t cr_bytes_for(uint64_t num_sides) { return num_sides * 128 + 64; }
+inline int choose_rank_layout(uint64_t free_b, uint64_t num_sides, uint64_t sample_b, uint64_t fixed_b, uint64_t headroom, bool force_compact) {
+	const uint64_t rest = sample_b + fixed_b + headroom;
+	if(!force_compact && num_sides * 128 + rank16_bytes_for(num_sides) + rest <= free_b) return kLayoutRank16;
+	if(cr_bytes_for(num_sides) + rest <= free_b) return kLayoutCompact;
+	return kLayoutNone;
+}
+
 CFB_HD int bwt_char(const IndexView& v, uint64_t row) {
 #ifdef __CUDA_ARCH__
 	if(v.rank16) {     // device replica: the indicator bits of the row's 64-row block (one 64-byte chunk); the '$' row has no bit and reads as A, as the file stores it
@@ -169,6 +262,7 @@ CFB_HD int bwt_char(const IndexView& v, uint64_t row) {
 		return (int)(bit(1) * 1 + bit(2) * 2 + bit(3) * 3);
 	}
 #endif
+	if(v.cr) return cr_bwt(v, row);
 	uint64_t s = row / 384; uint32_t off = (uint32_t)(row - s * 384);
 	return (int)((v.sides[s * 16 + (off >> 5)] >> ((off & 31) * 2)) & 3);
 }
@@ -183,6 +277,7 @@ CFB_HD uint64_t lf_scalar(const IndexView& v, uint64_t row, int c) {
 		return r16_lf(v, row, c, e[0], e[1]);
 	}
 #endif
+	if(v.cr) return cr_lf(v, row, c);
 	uint64_t s = row / 384; uint32_t off = (uint32_t)(row - s * 384);
 	const uint64_t* w = v.sides + s * 16;
 	uint32_t full = off >> 5, rem = off & 31;

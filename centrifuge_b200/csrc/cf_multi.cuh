@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(128) k_gather_probe(const unsigned long long* 
 	}
 	if(acc == 0x123456789abcull) *sink = acc;
 }
-// table: 0 = rank16 (16-byte entries), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it),
+// table: 0 = the loaded rank structure, rank16 or the compact layout (16-byte pieces), 1 = K-mer jump table (16-byte), 2 = walk8 (8-byte), 3 = resolve table (8-byte words of it),
 // 4 = death bits, which have no table of their own (always "not built")
 // ctas_per_sm CTAs of 128 threads per SM (all resident when <= 16), ilp independent requests per thread in flight
 extern "C" int cfb_gather_rate(const cfb_index* ix, int table, uint64_t n_requests, int ctas_per_sm, int ilp, double* g_requests_per_s, double* ms_out) {
@@ -241,7 +241,7 @@ extern "C" int cfb_gather_rate(const cfb_index* ix, int table, uint64_t n_reques
 	const cfb_index_tables& t = ix->tables; const IndexView& v = ix->view;
 	const unsigned long long* base = nullptr; uint64_t n = 0; int W = 1;
 	switch(table) {
-		case 0: base = (const unsigned long long*)v.rank16; n = t.rank16_bytes / 16; W = 2; break;
+		case 0: base = (const unsigned long long*)(v.cr ? v.cr : v.rank16); n = (v.cr ? t.sides_bytes : t.rank16_bytes) / 16; W = 2; break;
 		case 1: base = (const unsigned long long*)v.ftabk; n = t.ftabk_bytes / 16; W = 2; break;
 		case 2: base = (const unsigned long long*)v.walk8; n = t.walk8_bytes / 8; W = 1; break;
 		case 3: base = v.rtab32 ? (const unsigned long long*)v.rtab32 : (const unsigned long long*)v.rtab16; n = t.resolve_table_bytes / 8; W = 1; break;

@@ -172,6 +172,16 @@ __global__ void k_mark_boundaries(const uint64_t* brow, uint32_t n, uint64_t* r1
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if(i < n) atomicOr((unsigned long long*)&r16[(brow[i] >> 6) * 8], 1ull << 63);
 }
+// compact rank layout (format: cf_logic.h, cr_convert_side / cr_lf): the superblock table first, from the file's sides, then
+// one thread per side converts it in place
+__global__ void k_cr_superblocks(const uint64_t* sides, uint64_t num_sides, uint64_t zoff, uint64_t nsb, uint64_t* sb) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if(i < nsb) cr_sb_entry(sides, num_sides, zoff, i, sb + i * 4);
+}
+__global__ void k_cr_convert(uint64_t* sides, uint64_t num_sides, uint64_t zoff, const uint64_t* sb) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if(i < num_sides) cr_convert_side(sides, num_sides, zoff, sb, i);
+}
 __global__ void k_build_ftab2(IndexView v, uint64_t n, uint64_t* ftab2) {
 	const uint64_t fi = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if(fi >= n) return;
@@ -215,8 +225,9 @@ __device__ __forceinline__ uint32_t ftabk_death(uint64_t y, uint32_t e) {
 	return 3;
 }
 // One thread per K-mer walks the depth-3 tree of extensions; a 64-byte rank16 chunk carries the entries of all four bases of
-// a block, so every tree node costs one or two loads.
+// a block, so every tree node costs one or two loads.  On the compact rank layout the walk takes cr_lf instead.
 __device__ __forceinline__ void lf4(const IndexView& v, const ulonglong2* r16, uint64_t top, uint64_t bot, uint64_t t[4], uint64_t b[4]) {
+	if(v.cr) { for(int c = 0; c < 4; c++) { t[c] = cr_lf(v, top, c); b[c] = cr_lf(v, bot, c); } return; }
 	const ulonglong2* pt = r16 + r16_entry(top, 0); const ulonglong2* pb = r16 + r16_entry(bot, 0);
 	#pragma unroll
 	for(int c = 0; c < 4; c++) {
@@ -234,6 +245,7 @@ __global__ void __launch_bounds__(128) k_build_ftabk(IndexView v, int K, uint64_
 	uint64_t top = v.ftab2[f10 * 2], bot = v.ftab2[f10 * 2 + 1];
 	for(int j = fc; j < K && bot > top; j++) {
 		const int c = (int)((fk >> (2 * j)) & 3);
+		if(v.cr) { top = cr_lf(v, top, c); bot = cr_lf(v, bot, c); continue; }
 		const ulonglong2 tq = __ldg(r16 + r16_entry(top, c)), bq = __ldg(r16 + r16_entry(bot, c));
 		top = r16_lf(v, top, c, tq.x, tq.y);
 		bot = r16_lf(v, bot, c, bq.x, bq.y);
@@ -556,9 +568,12 @@ struct UnitArgs {
 // twin the CPU tests pin against the oracle) would produce, but reached the way k_search_t reaches them -- K-mer jump, one
 // rank16 entry per step when top and bot share a block, eight bases per walk8 gather of the range's end rows -- so that regenerating
 // a list costs ~30 dependent gathers instead of ~250.  Used by k_prep (lists whose short hits matter) and k_search_long.
-// One partial search from `cur` (partial_search_scalar's result) with the device tables.
+// One partial search from `cur` (partial_search_scalar's result) with the device tables.  CR: on the compact rank layout (v.cr)
+// every LF step is cr_lf, and *nreq (when given) counts its 32-byte sector pieces.  Callers pick the instantiation once per
+// kernel or walk, so the rank16 one is the walk it always was.
+template <bool CR>
 __device__ __forceinline__ void partial_search_dev(const IndexView& v, const uint8_t* fw, uint32_t len, int strand, uint32_t cur,
-                                                   HitRec& h, uint32_t& new_cur, bool& done) {
+                                                   HitRec& h, uint32_t& new_cur, bool& done, unsigned long long* nreq = nullptr) {
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(v.rank16);
 	const ulonglong2* ftab2 = reinterpret_cast<const ulonglong2*>(v.ftab2);
 	const ulonglong2* ftabk = reinterpret_cast<const ulonglong2*>(v.ftabk);
@@ -594,6 +609,18 @@ __device__ __forceinline__ void partial_search_dev(const IndexView& v, const uin
 							if((st & sb) == 8u) { top = et & kWalkRowMask; bot = (eb & kWalkRowMask) + 1; dep += 8; continue; }
 							slow_until = dep + walk8_retry(st, sb);
 						}
+						if(CR) {
+							if(nreq) *nreq += 1 + ((top % kCrRows) > 64) + (bot - top == 1 ? 0 : 1 + ((bot % kCrRows) > 64));
+							if(bot - top == 1) {
+								if(top == v.zoff || cr_bwt(v, top) != c) break;            // mapLF1: BWT[top] must be c, and not the '$' stored as A
+								top = cr_lf(v, top, c); bot = top + 1; dep++;
+							} else {
+								const uint64_t t = cr_lf(v, top, c), b = cr_lf(v, bot, c);
+								if(b <= t) break;
+								top = t; bot = b; dep++;
+							}
+							continue;
+						}
 						if(bot - top == 1) {
 							const ulonglong2 e = __ldg(r16 + r16_entry(top, c));
 							if(!((e.y >> (top & 63)) & 1ull)) break;                      // mapLF1: BWT[top] must be c ('$' has no bit)
@@ -612,12 +639,14 @@ __device__ __forceinline__ void partial_search_dev(const IndexView& v, const uin
 		}
 	}
 }
-__device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t len, int strand, HitRec* hits, uint32_t cap) {
+template <bool CR>
+__device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const uint8_t* fw, uint32_t len, int strand, HitRec* hits, uint32_t cap,
+                                      unsigned long long* nreq = nullptr) {
 	uint32_t cur = 0, n = 0;
 	if(len == 0) return 0;
 	for(;;) {
 		HitRec h; uint32_t new_cur; bool done;
-		partial_search_dev(v, fw, len, strand, cur, h, new_cur, done);
+		partial_search_dev<CR>(v, fw, len, strand, cur, h, new_cur, done, nreq);
 		if(n < cap) hits[n] = h;
 		n++;
 		cur = new_cur;
@@ -631,12 +660,14 @@ __device__ uint32_t search_strand_dev(const IndexView& v, const Params& p, const
 // k_search_long: batches with a read longer than k_search_t's widest register window (kWindowLen bases).  One thread per
 // (unit, mate, strand) task runs the strand's whole search from the byte form of the read and stores every hit, so k_prep
 // never regenerates these lists.  SCALAR runs search_strand_scalar, one LF step at a time with the jump tables off, for every read
-// length: the pass that counts the reference's operations (SURVEY 8d).  The table walk counts no load requests for these reads.
+// length: the pass that counts the reference's operations (SURVEY 8d).  On rank16 the table walk counts no load requests for these
+// reads; on the compact rank layout, where this kernel serves every read length, CFB_COUNT=2 counts its sector pieces in req_rank16.
 static const uint32_t kWindowLen = 320;      // 10 register words of 32 bases
-template <bool SCALAR>
+template <bool SCALAR, bool CR = false>
 __global__ void __launch_bounds__(kSearchThreads) k_search_long(const SearchArgs a) {
 	const uint32_t per = 2u * (uint32_t)a.b.n_mates;
 	Counters local; memset(&local, 0, sizeof local);
+	unsigned long long* nreq = !SCALAR && CR && a.ctr ? &local.req_rank16 : nullptr;
 	for(uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x; tid < a.ntasks; tid += gridDim.x * blockDim.x) {
 		const uint32_t unit = tid / per, rem = tid - unit * per;
 		const int mate = (int)(rem >> 1), strand = (int)(rem & 1);
@@ -646,7 +677,7 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_long(const SearchArgs
 		const uint8_t* fw = a.b.bases + a.b.off[mate][unit];
 		HitRec* hits = a.hits + (size_t)tid * a.cap;
 		const uint32_t n = SCALAR ? search_strand_scalar(a.v, a.p, fw, len, strand, hits, a.cap, &local)
-		                          : search_strand_dev(a.v, a.p, fw, len, strand, hits, a.cap);
+		                          : search_strand_dev<CR>(a.v, a.p, fw, len, strand, hits, a.cap, nreq);
 		if(n > a.cap) atomicExch(a.overflow, 1u);      // the host grows the lists and re-runs the batch
 		a.nhits[tid] = nh_pack(min(n, a.cap), n, false);
 	}
@@ -654,13 +685,16 @@ __global__ void __launch_bounds__(kSearchThreads) k_search_long(const SearchArgs
 		atomicAdd(&a.ctr->partial_searches, local.partial_searches); atomicAdd(&a.ctr->ftab_probes, local.ftab_probes);
 		atomicAdd(&a.ctr->sides_search, local.sides_search); atomicAdd(&a.ctr->lf_steps, local.lf_steps);
 	}
+	if(nreq && local.req_rank16) atomicAdd(&a.ctr->req_rank16, local.req_rank16);
 }
 
 typedef void (*SearchKernel)(const SearchArgs);
 // count 1: the scalar search, which counts the reference's operations; otherwise the thread-per-walk kernel whose register
-// window holds the batch's longest read (count 2: its request-counting instantiation)
-static SearchKernel search_kernel(uint32_t maxlen, int count) {
+// window holds the batch's longest read (count 2: its request-counting instantiation).  k_search_t reads rank16 only: on the
+// compact rank layout every batch takes the thread-per-walk kernel.
+static SearchKernel search_kernel(uint32_t maxlen, int count, bool compact) {
 	if(count == 1) return k_search_long<true>;
+	if(compact) return k_search_long<false, true>;
 	if(maxlen > kWindowLen) return k_search_long<false>;
 	const bool reqs = count == 2;
 	if(maxlen > 160) return reqs ? k_search_t<true, 10> : k_search_t<false, 10>;
@@ -720,7 +754,8 @@ __global__ void __launch_bounds__(128, MINB) k_prep(const UnitArgs a) {
 					const unsigned long long slot = atomicAdd(a.regen_ctr, 1ull);
 					if(slot >= a.regen_slots) { atomicExch(a.overflow, 4u); continue; }      // the host grows the side buffer and re-runs the batch
 					HitRec* L = a.regen + (size_t)slot * a.full_cap;
-					const uint32_t n = search_strand_dev(a.v, a.p, fw[r], u.rdlen[r], st, L, a.full_cap);
+					const uint32_t n = a.v.cr ? search_strand_dev<true>(a.v, a.p, fw[r], u.rdlen[r], st, L, a.full_cap)
+					                          : search_strand_dev<false>(a.v, a.p, fw[r], u.rdlen[r], st, L, a.full_cap);
 					if(n > a.full_cap) atomicExch(a.overflow, 1u);
 					u.L[r][st] = L; u.n[r][st] = min(n, a.full_cap);
 					a.regen_n[slot] = u.n[r][st]; a.nhits[tpos[r] + st] = kListRegen | (uint32_t)slot;
@@ -894,8 +929,10 @@ __device__ __forceinline__ int group_lf(const IndexView& v, uint64_t row, const 
 // at the row knows BWT[row] and its own LF value is the next row.  The genome-boundary prefilter is the
 // flag bit in A's occ word (no separate bitmap load).
 // ---------------------------------------------------------------------------------------
-// IDENT: rows are 0..n-1 themselves and results go to the (16- or 32-bit) resolve table -- used once at index load
-template <bool COUNT, bool IDENT>
+// IDENT: rows are 0..n-1 themselves and results go to the (16- or 32-bit) resolve table -- used once at index load.
+// CR: the compact rank layout.  The four lanes of a group step together through cr_bwt / cr_lf of the same row (their loads
+// coalesce), and boundary rows are found through the .4.cf bitmap (bbits), as rank16's boundary flag has no place there.
+template <bool COUNT, bool IDENT, bool CR = false>
 __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs a) {
 	const unsigned lane = threadIdx.x & 31, gl = lane & 3, gbase = lane & 28, gmask = 0xFu << gbase;
 	const ulonglong2* r16 = reinterpret_cast<const ulonglong2*>(a.v.rank16);
@@ -928,11 +965,13 @@ __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs 
 		}
 		if(!__any_sync(0xffffffffu, mode != R_DONE)) break;
 		ulonglong2 e = make_ulonglong2(0, 0); uint32_t samp = 0;
-		if(mode == R_WALK) e = __ldg(r16 + r16_entry(row, (int)gl));
+		if(mode == R_WALK && !CR) e = __ldg(r16 + r16_entry(row, (int)gl));
 		else if(mode == R_SAMPLE && gl == 0) samp = a.v.sample32 ? __ldg(a.v.sample32 + (row >> a.v.off_rate)) : (uint32_t)__ldg(a.v.sample16 + (row >> a.v.off_rate));
 		if(mode == R_SAMPLE) { if(gl == 0) put(samp); mode = R_NEED; }
 		else if(mode == R_WALK) {
-			const unsigned flagged = __shfl_sync(gmask, (unsigned)(e.x >> 63), gbase);     // A's entry carries the boundary flag
+			unsigned flagged = 0;
+			if(CR) { if(a.v.n_boundaries && row <= a.v.last_boundary) { const uint64_t b = row >> a.v.bshift; flagged = (a.v.bbits[b >> 5] >> (b & 31)) & 1u; } }
+			else flagged = __shfl_sync(gmask, (unsigned)(e.x >> 63), gbase);     // A's entry carries the boundary flag
 			bool found = false;
 			if(flagged && a.v.last_boundary > 0 && row <= a.v.last_boundary) {
 				uint32_t lo = 0, hi = a.v.n_boundaries;
@@ -941,7 +980,8 @@ __global__ void __launch_bounds__(kSearchThreads) k_resolve_c(const ResolveArgs 
 			}
 			if(found) mode = R_NEED;
 			else {
-				group_lf(a.v, row, e, row);      // exactly one base owns the row: settle() took the '$' row
+				if(CR) row = cr_lf(a.v, row, cr_bwt(a.v, row));
+				else group_lf(a.v, row, e, row);      // exactly one base owns the row: settle() took the '$' row
 				if(COUNT && gl == 0) c_walk++;
 				mode = settle(row);
 			}
@@ -1020,9 +1060,9 @@ struct LongArgs {
 	unsigned long long* stats;                      // [0] speculative partial searches, [1] re-searched at the join
 	UnitArgs u;
 };
-struct DevStep {
+template <bool CR> struct DevStep {
 	const IndexView& v; const uint8_t* fw; uint32_t len; int strand; unsigned long long n;
-	__device__ void operator()(uint32_t cur, HitRec& h, uint32_t& nc, bool& done) { partial_search_dev(v, fw, len, strand, cur, h, nc, done); n++; }
+	__device__ void operator()(uint32_t cur, HitRec& h, uint32_t& nc, bool& done) { partial_search_dev<CR>(v, fw, len, strand, cur, h, nc, done); n++; }
 };
 struct ScalarStep {      // CFB_COUNT=1: the scalar search, counting the reference's operations
 	const IndexView& v; const uint8_t* fw; uint32_t len; int strand; Counters* ctr;
@@ -1041,10 +1081,10 @@ __global__ void __launch_bounds__(128) k_long_seg(const LongArgs a) {
 		while(hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if(a.tasks[mid].soff <= g) lo = mid; else hi = mid; }
 		const LongTask t = a.tasks[lo];
 		const uint32_t local = (uint32_t)(g - t.soff), strand = local / t.nseg, k = local - strand * t.nseg;
-		DevStep step{a.v, long_fw(a, t), t.len, (int)strand, 0ull};
 		const uint32_t start = k * kSegLen, stop = min(start + kSegLen, t.len);
-		a.sn[g] = seg_chain(a.p, t.len, start, stop, step, a.seg + t.hoff + (uint64_t)strand * t.len + start, a.sexit + g);
-		n = step.n;
+		HitRec* out = a.seg + t.hoff + (uint64_t)strand * t.len + start;
+		if(a.v.cr) { DevStep<true> step{a.v, long_fw(a, t), t.len, (int)strand, 0ull}; a.sn[g] = seg_chain(a.p, t.len, start, stop, step, out, a.sexit + g); n = step.n; }
+		else { DevStep<false> step{a.v, long_fw(a, t), t.len, (int)strand, 0ull}; a.sn[g] = seg_chain(a.p, t.len, start, stop, step, out, a.sexit + g); n = step.n; }
 	}
 	for(int d = 16; d > 0; d >>= 1) n += __shfl_xor_sync(0xffffffffu, n, d);
 	if((threadIdx.x & 31) == 0 && n) atomicAdd(&a.stats[0], n);
@@ -1066,10 +1106,11 @@ __global__ void __launch_bounds__(128) k_long_join(const LongArgs a) {
 		atomicAdd(&a.u.ctr->sides_search, local.sides_search); atomicAdd(&a.u.ctr->lf_steps, local.lf_steps);
 		return;
 	}
-	DevStep step{a.v, fw, t.len, strand, 0ull};
 	const uint64_t s0 = t.soff + (uint64_t)strand * t.nseg;
+	const HitRec* seg = a.seg + t.hoff + (uint64_t)strand * t.len;
 	unsigned long long re = 0;
-	a.nh[i] = seg_join(a.p, t.len, kSegLen, a.seg + t.hoff + (uint64_t)strand * t.len, a.sn + s0, a.sexit + s0, step, out, &re);
+	if(a.v.cr) { DevStep<true> step{a.v, fw, t.len, strand, 0ull}; a.nh[i] = seg_join(a.p, t.len, kSegLen, seg, a.sn + s0, a.sexit + s0, step, out, &re); }
+	else { DevStep<false> step{a.v, fw, t.len, strand, 0ull}; a.nh[i] = seg_join(a.p, t.len, kSegLen, seg, a.sn + s0, a.sexit + s0, step, out, &re); }
 	if(re) atomicAdd(&a.stats[1], re);
 }
 
@@ -1267,6 +1308,23 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 		ix->sm_count = prop.multiProcessorCount;
 		IndexView& v = ix->view; memset(&v, 0, sizeof v);
 		int rc;
+		// The rank layout, chosen before anything is allocated (choose_rank_layout): rank16 (1 byte per row, built beside the
+		// streamed sides, which it replaces) when it fits with everything else, else the compact layout (1/3 byte per row, built in
+		// place from the sides).  Head-room as for the derived tables below.  CFB_RANK16=0 forces the compact layout (tests, A/B).
+		size_t free0 = 0, total0 = 0; cudaMemGetInfo(&free0, &total0);
+		double head_gb = 12.0; { const char* e = getenv("CFB_HBM_HEADROOM_GB"); if(e) head_gb = atof(e); }
+		const uint64_t headroom0 = std::min<uint64_t>((uint64_t)(head_gb * 1073741824.0), free0 / 2);
+		const uint64_t sample_b = h.offs_len * (h.wide_sample ? 4 : 2);
+		const uint64_t fixed_b = (h.ftab.size() + h.eftab.size() + h.brow.size() + h.seq_taxid.size() + h.paths.size()) * 8
+		                       + (h.bseq.size() + h.bbits.size() + h.seq_path.size()) * 4 + (h.ftab_len - 1) * 16 + cr_superblocks(h.num_sides) * 32;
+		const char* er = getenv("CFB_RANK16");
+		const int layout = choose_rank_layout(free0, h.num_sides, sample_b, fixed_b, headroom0, er && er[0] == '0');
+		if(layout == kLayoutNone) {
+			const unsigned long long nr = rank16_bytes_for(h.num_sides) + h.num_sides * 128, nc = cr_bytes_for(h.num_sides), rest = sample_b + fixed_b + headroom0;
+			delete ix;
+			return fail(CFB_ENOMEM, "index %s fits no rank layout on device %d: rank16 needs %llu bytes and the compact layout %llu, each plus %llu bytes "
+			            "of sample, fixed tables and head-room; %llu bytes are free", basename, device, nr + rest, nc + rest, rest, (unsigned long long)free0);
+		}
 		#define UP(field, vec, T) if((rc = upload(ix, (vec).data(), (vec).size() * sizeof(T), (const void**)&v.field)) != CFB_OK) { cfb_index_free(ix); return rc; }
 		if((rc = stream_to_device(ix, std::string(basename) + ".1.cf", h.sides_file_off, h.num_sides * h.side_sz, (const void**)&v.sides)) != CFB_OK) { cfb_index_free(ix); return rc; }
 		ix->tables.sample_bytes = h.offs_len * (h.wide_sample ? 4 : 2);
@@ -1282,23 +1340,40 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 		v.n_boundaries = (uint32_t)h.brow.size(); v.n_seqs = (uint32_t)h.seq_taxid.size();
 		v.off_rate = h.off_rate; v.ftab_chars = h.ftab_chars; v.bshift = h.bshift;
 		{   // 16-byte rank entries + fused ftab for the walk kernels
+			const bool compact = layout == kLayoutCompact;
 			uint64_t* r16 = nullptr; const uint64_t nb = h.num_sides * 6;
-			CKX(cudaMalloc((void**)&r16, (nb + 1) * 64));
-			ix->dptrs.push_back(r16); ix->device_bytes += (nb + 1) * 64;
-			k_build_rank16<<<(unsigned)((nb + 1 + 255) / 256), 256>>>(v.sides, h.num_sides, v.zside, v.zoffc, r16);
-			if(v.n_boundaries) k_mark_boundaries<<<(v.n_boundaries + 255) / 256, 256>>>(v.brow, v.n_boundaries, r16);
+			if(compact) {
+				const uint64_t nsb = cr_superblocks(h.num_sides);
+				uint64_t* sb = nullptr;
+				CKX(cudaMalloc((void**)&sb, nsb * 32));
+				ix->dptrs.push_back(sb); ix->device_bytes += nsb * 32;
+				k_cr_superblocks<<<(unsigned)((nsb + 255) / 256), 256>>>(v.sides, h.num_sides, h.zoff, nsb, sb);
+				k_cr_convert<<<(unsigned)((h.num_sides + 255) / 256), 256>>>(const_cast<uint64_t*>(v.sides), h.num_sides, h.zoff, sb);
+				v.crsb = sb;
+			} else {
+				CKX(cudaMalloc((void**)&r16, (nb + 1) * 64));
+				ix->dptrs.push_back(r16); ix->device_bytes += (nb + 1) * 64;
+				k_build_rank16<<<(unsigned)((nb + 1 + 255) / 256), 256>>>(v.sides, h.num_sides, v.zside, v.zoffc, r16);
+				if(v.n_boundaries) k_mark_boundaries<<<(v.n_boundaries + 255) / 256, 256>>>(v.brow, v.n_boundaries, r16);
+			}
 			uint64_t* f2 = nullptr; const uint64_t nf = h.ftab_len - 1;
 			CKX(cudaMalloc((void**)&f2, nf * 16));
 			ix->dptrs.push_back(f2); ix->device_bytes += nf * 16;
 			k_build_ftab2<<<(unsigned)((nf + 255) / 256), 256>>>(v, nf, f2);
 			CKX(cudaDeviceSynchronize());
-			v.rank16 = r16; v.ftab2 = f2;
-			ix->tables.rank16_bytes = (nb + 1) * 64; ix->tables.ftab2_bytes = nf * 16;
-			// The file's sides were only the staging buffer of rank16, which holds the same information (the scalar LF of the
-			// extension step reads rank16 too): no kernel reads them from here on.
-			cudaFree((void*)v.sides);
-			ix->dptrs.erase(std::find(ix->dptrs.begin(), ix->dptrs.end(), (void*)v.sides));
-			ix->device_bytes -= h.num_sides * h.side_sz; v.sides = nullptr;
+			v.ftab2 = f2; ix->tables.ftab2_bytes = nf * 16;
+			if(compact) {      // the converted sides are the rank structure: sides_bytes reports them
+				v.cr = v.sides; v.sides = nullptr;
+				ix->tables.sides_bytes = cr_bytes_for(h.num_sides);
+			} else {
+				v.rank16 = r16;
+				ix->tables.rank16_bytes = (nb + 1) * 64;
+				// The file's sides were only the staging buffer of rank16, which holds the same information (the scalar LF of the
+				// extension step reads rank16 too): no kernel reads them from here on.
+				cudaFree((void*)v.sides);
+				ix->dptrs.erase(std::find(ix->dptrs.begin(), ix->dptrs.end(), (void*)v.sides));
+				ix->device_bytes -= h.num_sides * h.side_sz; v.sides = nullptr;
+			}
 			// HBM budget of the derived tables: what is free now minus the head-room the batch buffers need (12 GB by default, 15 % of an
 			// 80 GB H100: 4 slots of 0.5 M 100 bp reads in flight at ~3 KB each with 30 % to grow,
 			// plus 3 GB of fixed buffers; callers that keep more in flight set CFB_HBM_HEADROOM_GB, as bench.py does).  Tables are built in the order of gathers saved per
@@ -1307,7 +1382,6 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 			// range jumps, K = 14 (4.3 GB, walk8 on 34 % of the bench index's rows instead of 16 %) measured the same as K = 15
 			// (274.5 vs 274.6-275.7 M reads/s on one H100 80GB HBM3 at 400 W), so the K-mer table keeps its place in the order.
 			size_t free_b = 0, total_b = 0; cudaMemGetInfo(&free_b, &total_b);
-			double head_gb = 12.0; { const char* e = getenv("CFB_HBM_HEADROOM_GB"); if(e) head_gb = atof(e); }
 			const uint64_t headroom = std::min<uint64_t>((uint64_t)(head_gb * 1073741824.0), free_b / 2);
 			auto budget = [&]() -> uint64_t { size_t f = 0, t = 0; cudaMemGetInfo(&f, &t); return f > headroom ? f - headroom : 0; };
 			// K-mer jump table with its death bitmap: K = largest value with 4^K <= len/4 (most K-mers occur), capped at 15 and by
@@ -1331,8 +1405,9 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 					ix->tables.ftabk_bytes = nk * 16; ix->tables.ftabk_chars = K; ix->tables.ftabd_chars = v.ftabd_chars;
 				}
 			}
-			// resolve table: sequence id of every SA row (walked once here)
-			{
+			// resolve table: sequence id of every SA row (walked once here).  Neither it nor walk8 is built on the compact layout: at the
+			// sizes that need it they would not fit, and they never change results.
+			if(!compact) {
 				const char* e = (flags & CFB_LOAD_NO_RESOLVE_TABLE) ? "0" : getenv("CFB_RESOLVE_TABLE");
 				const uint64_t nrows = h.len + 1, esz = h.wide_sample ? 4 : 2;
 				if(!(e && e[0] == '0') && nrows * esz + 16 <= budget()) {
@@ -1352,7 +1427,7 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 				}
 			}
 			// walk8: eight single-row LF steps per gather, for as many rows as the budget allows (at least an eighth of them)
-			{
+			if(!compact) {
 				const char* e = (flags & CFB_LOAD_NO_WALK8) ? "0" : getenv("CFB_WALK8");
 				const uint64_t nrows = h.len + 1;
 				uint64_t cover = std::min<uint64_t>(nrows, budget() / 8);
@@ -1895,8 +1970,8 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	// which search kernel runs decides what it stores: k_search_t keeps only hits of >= kLongLen bases when min_hitlen allows
 	// it (see kListRegen); k_search_long -- for long reads, and the scalar search of a CFB_COUNT=1 pass at any read length --
 	// and small min_hitlen keep every hit
-	const SearchKernel search = search_kernel(s.maxlen, c->count);
-	const bool keep_short = search == k_search_long<true> || search == k_search_long<false> || c->prm.min_hitlen < kLongLen || c->keep_short;
+	const SearchKernel search = search_kernel(s.maxlen, c->count, c->view.cr != nullptr);
+	const bool keep_short = search == k_search_long<true> || search == k_search_long<false> || search == k_search_long<false, true> || c->prm.min_hitlen < kLongLen || c->keep_short;
 	if(stage == 0) {
 		if(s.cap == 0) {
 			s.full_cap = s.maxlen / 4 + 8;      // >= #Ns allowed by the N filter (0.15 len) + len/10 + slack
@@ -1978,6 +2053,7 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	ResolveArgs ra; ra.v = c->view; ra.rows = s.rows.p; ra.ids = s.ids.p; ra.ids16 = nullptr; ra.total = (const uint64_t*)(s.scal.p + 3); ra.rows_cap = s.rows_cap;
 	ra.task_ctr = s.scal.p + 1; ra.chunk = 64; ra.ctr = ctr;
 	if((c->view.rtab16 || c->view.rtab32) && c->count != 1) k_lookup<<<c->ix->sm_count * 8, 256, 0, s.st>>>(ra);
+	else if(c->view.cr) { if(c->count) k_resolve_c<true, false, true><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra); else k_resolve_c<false, false, true><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra); }
 	else if(c->count) k_resolve_c<true, false><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra);
 	else k_resolve_c<false, false><<<c->resolve_blocks, kSearchThreads, 0, s.st>>>(ra);
 	c->launches++;
@@ -2212,7 +2288,8 @@ extern "C" int cfb_test_resolve(const cfb_index* ix, const uint64_t* rows, uint6
 	unsigned long long init[2] = {0ull, (unsigned long long)n};
 	CK(cudaMemcpy(sc, init, 16, cudaMemcpyHostToDevice));
 	ResolveArgs ra; ra.v = ix->view; ra.rows = dr; ra.ids = dout; ra.ids16 = nullptr; ra.total = (const uint64_t*)(sc + 1); ra.rows_cap = n; ra.task_ctr = sc; ra.chunk = 64; ra.ctr = nullptr;
-	k_resolve_c<false, false><<<32, kSearchThreads>>>(ra);
+	if(ix->view.cr) k_resolve_c<false, false, true><<<32, kSearchThreads>>>(ra);
+	else k_resolve_c<false, false><<<32, kSearchThreads>>>(ra);
 	CK(cudaDeviceSynchronize());
 	CK(cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost));
 	cudaFree(dr); cudaFree(dout); cudaFree(sc);

@@ -70,7 +70,9 @@ int cfb_index_get_info(const cfb_index*, cfb_index_info* out);
  * this order of benefit per byte, each only while it fits the budget left after the batch head-room (12 GB unless
  * CFB_HBM_HEADROOM_GB says otherwise; DESIGN.md 3): rank16 + ftab2 (always), the K-mer jump table (whose 16-byte entries
  * also carry the death bitmap), the resolve table, walk8 (possibly for a prefix of the rows).  The file's sides only stage
- * rank16 and are freed once it is built, so sides_bytes is always 0. */
+ * rank16 and are freed once it is built, so sides_bytes is 0 for a rank16 replica.  When rank16 does not fit, the sides are
+ * converted in place into the compact rank layout (1/3 byte per row), which sides_bytes then reports with rank16_bytes = 0;
+ * such a replica has no resolve table and no walk8 (DESIGN.md 3). */
 typedef struct {
 	uint64_t sides_bytes, sample_bytes, rank16_bytes, ftab2_bytes, ftabk_bytes, resolve_table_bytes, walk8_bytes;
 	uint64_t total_bytes, free_bytes_after_load;
