@@ -688,6 +688,55 @@ template <class T, class C> CFB_HDN void std_sort(T* first, T* last, C comp) {
 }
 
 // ----------------------------------------------------------------------------------------
+// What the rank16 search path leaves out of its hit lists, and when k_prep must put it back.
+// nhits[] word of a strand list: hits stored (15 bits) | hits found (15 bits, saturating) << 15 | kListNoLong.  With
+// min_hitlen >= kLongLen k_search_t stores only hits of at least kLongLen bases: shorter ones are never counted
+// (classifier.h:299), sort after every stored hit (compareBWTHits puts len >= 22 first) and touch nothing else -- unless
+// both strands of a mate are in play (extension / twin removal, classifier.h:790-870) or a list is long enough for
+// introsort (> 16 hits, where libstdc++'s tie permutation may depend on every element).  In those cases k_prep regenerates
+// the full list (list_needs_regen) into a side buffer and points the list at it: word = kListRegen | slot.  Nine of ten hits
+// of a typical read are short, so this removes most of the hit traffic and shrinks the per-read device footprint.
+// Hits the death bitmap of the K-mer table ends (at most K + 2 bases, only while min_hitlen >= K + 3) are stored with
+// top = bot = kUnk, so their size reads as 0; list_needs_exact_ranges says where k_prep must recompute them.
+// ----------------------------------------------------------------------------------------
+static const uint32_t kListNoLong = 0x80000000u;             // the strand has no hit of min_hitlen bases
+static const uint32_t kListRegen = 0x40000000u;              // the list lives in the regeneration buffer, slot = low 30 bits (written by k_prep)
+static const uint32_t kLongLen = 22;
+CFB_HD uint32_t nh_pack(uint32_t stored, uint32_t found, bool nolong) {
+	return (stored & 0x7fffu) | ((found < 0x7fffu ? found : 0x7fffu) << 15) | (nolong ? kListNoLong : 0u);
+}
+CFB_HD uint32_t nh_stored(uint32_t w) { return w & 0x7fffu; }
+CFB_HD uint32_t nh_found(uint32_t w) { return (w >> 15) & 0x7fffu; }
+
+// Whether load_unit empties strand list st of a mate whose nhits words are raw[0], raw[1].  A strand list without a hit of
+// min_hitlen bases matters only to the extension step, which needs such a hit on BOTH strands (classifier.h:790-802);
+// everything later (trimming within a list, strand choice, counting, scoring) ignores or only shortens short hits.  So unless
+// both strands have one, such a list is never read.
+CFB_HD bool list_dropped(const uint32_t raw[2], int st) {
+	return !((raw[0] | raw[1]) & kListRegen) && (raw[st] & kListNoLong);
+}
+// Whether k_prep regenerates a list that holds only the long hits: n hits stored, n_other in the mate's other strand list
+// (after load_unit), `found` hits found by the search.
+CFB_HD bool list_needs_regen(uint32_t n, uint32_t n_other, uint32_t found) {
+	return n > 0 && (n_other > 0 || found > 16);
+}
+// Whether k_prep gives the kUnk hits of a list their exact SA ranges.  A short hit's range can matter
+//  - through the twin removal (both strands in play, classifier.h:850-870);
+//  - through libstdc++'s tie permutation in lists long enough for introsort (> 16 hits);
+//  - through the time stamps, when the list holds a counted hit shorter than kLongLen (only with min_hitlen < 21): such a hit
+//    is ordered by size / len among the uncounted short hits (compareBWTHits), so a kUnk hit (size 0) can sort ahead of it.
+//    EmitRows advances ts for every hit of a list, counted or not, and after a list left through its `break` the next
+//    list's first counted hit shares the previous one's time stamp only at index 0 (kRowSameTs) -- which moves the scores.
+// With min_hitlen >= kLongLen - 1 no counted hit is shorter than kLongLen, and the rule is the first two cases alone.
+CFB_HD bool list_needs_exact_ranges(const Params& p, const HitRec* L, uint32_t n, uint32_t n_other) {
+	if(n == 0) return false;
+	if(n_other > 0 || n > 16) return true;
+	if(p.min_hitlen + 1 >= kLongLen) return false;
+	for(uint32_t i = 0; i < n; i++) if(L[i].len > p.min_hitlen && L[i].len < kLongLen) return true;
+	return false;
+}
+
+// ----------------------------------------------------------------------------------------
 // Resolve planning + scoring
 // ----------------------------------------------------------------------------------------
 struct UnitHits {      // hit lists of one unit: [mate][strand]

@@ -96,11 +96,6 @@ OPTS = {"default": {}, "k1_minhit15": {"k": 1, "min_hitlen": 15}}
 TABLES = {"kmer_default": {}, "kmer_at_ftab": {"CFB_FTABK": "FC"}, "no_bitmap": {"CFB_FTABD": "0"}}
 
 
-# rank16's records differ from the oracle's in score on these cases (indexes built with other --ftabchars / --offrate values, pairs,
-# -k 1 --min-hitlen 15); the compact layout gives the oracle's.  A discrepancy of the rank16 search path, left to be fixed there.
-RANK16_OFF_ORACLE = {(n, "pe", "k1_minhit15") for n in ("adv_t1o2", "adv_t6o0", "adv_t8o7")}
-
-
 @pytest.mark.parametrize("tables", sorted(TABLES))
 @pytest.mark.parametrize("name", INDEXES)
 def test_compact_records_equal_rank16_and_oracle(name, tables, monkeypatch):
@@ -128,8 +123,6 @@ def test_compact_records_equal_rank16_and_oracle(name, tables, monkeypatch):
             assert_same(on, orec, gn, grec)
         except AssertionError as e:
             raise AssertionError("%s %s %s %s: compact vs oracle: %s" % (name, tables, rs, opt, e))
-        if (name, rs, opt) in RANK16_OFF_ORACLE:
-            continue
         try:
             assert_same(wn, wrec, gn, grec)
         except AssertionError as e:
