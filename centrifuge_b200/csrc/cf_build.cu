@@ -14,6 +14,7 @@
 #include "../../include/cfb200.h"
 #include "cf_index.h"
 #include "cf_synth.h"
+#include "cf_buf.cuh"
 
 #include <cub/cub.cuh>
 
@@ -407,13 +408,6 @@ static std::string write_cf3(const std::string& base, const Meta& m, const cfb_b
 	return "";
 }
 
-template <class T> struct Dev {
-	T* p = nullptr; size_t n = 0;
-	cudaError_t alloc(size_t k) { release(); n = k; return cudaMalloc((void**)&p, (k ? k : 1) * sizeof(T)); }
-	void release() { if(p) cudaFree(p); p = nullptr; n = 0; }
-	~Dev() { release(); }
-};
-
 }  // namespace
 
 extern "C" const char* cfb_build_last_error(void) { return g_berr.c_str(); }
@@ -462,10 +456,10 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 
 	// ---- text on the device
 	const uint64_t nwords = (len + 31) / 32 + 4;
-	Dev<uint64_t> text; BCK(text.alloc(nwords)); BCK(cudaMemset(text.p, 0, nwords * 8));
+	DBuf<uint64_t> text; BCK(text.alloc(nwords)); BCK(cudaMemset(text.p, 0, nwords * 8));
 	if(synth) { k_synth_text<<<(unsigned)((nwords + 255) / 256), 256>>>(sp, text.p, (len + 31) / 32, len); }
 	else {
-		Dev<uint8_t> dc; BCK(dc.alloc(len)); BCK(cudaMemcpy(dc.p, codes.data(), len, cudaMemcpyHostToDevice));
+		DBuf<uint8_t> dc; BCK(dc.alloc(len)); BCK(cudaMemcpy(dc.p, codes.data(), len, cudaMemcpyHostToDevice));
 		k_pack_text<<<(unsigned)(((len + 31) / 32 + 255) / 256), 256>>>(dc.p, len, text.p, (len + 31) / 32);
 		BCK(cudaDeviceSynchronize());
 		std::vector<uint8_t>().swap(codes);
@@ -473,19 +467,19 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 	BCK(cudaDeviceSynchronize());
 
 	// ---- global outputs
-	Dev<uint32_t> bwt; BCK(bwt.alloc(num_sides * 24)); BCK(cudaMemset(bwt.p, 0, num_sides * 24 * 4));
-	Dev<uint32_t> sample; BCK(sample.alloc(offs_len)); BCK(cudaMemset(sample.p, 0, offs_len * 4));
-	Dev<unsigned long long> ftab_cnt; BCK(ftab_cnt.alloc(ftab_len + 1)); BCK(cudaMemset(ftab_cnt.p, 0, (ftab_len + 1) * 8));
-	Dev<uint32_t> markbits; BCK(markbits.alloc(len / 32 + 2)); BCK(cudaMemset(markbits.p, 0, (len / 32 + 2) * 4));
+	DBuf<uint32_t> bwt; BCK(bwt.alloc(num_sides * 24)); BCK(cudaMemset(bwt.p, 0, num_sides * 24 * 4));
+	DBuf<uint32_t> sample; BCK(sample.alloc(offs_len)); BCK(cudaMemset(sample.p, 0, offs_len * 4));
+	DBuf<unsigned long long> ftab_cnt; BCK(ftab_cnt.alloc(ftab_len + 1)); BCK(cudaMemset(ftab_cnt.p, 0, (ftab_len + 1) * 8));
+	DBuf<uint32_t> markbits; BCK(markbits.alloc(len / 32 + 2)); BCK(cudaMemset(markbits.p, 0, (len / 32 + 2) * 4));
 	{
 		std::vector<uint32_t> hb(len / 32 + 2, 0);
 		for(size_t i = 0; i < m.mark_pos.size(); i++) hb[m.mark_pos[i] >> 5] |= 1u << (m.mark_pos[i] & 31);
 		BCK(cudaMemcpy(markbits.p, hb.data(), hb.size() * 4, cudaMemcpyHostToDevice));
 	}
 	const uint32_t bound_cap = (uint32_t)m.mark_pos.size() + 16;
-	Dev<uint64_t> bound_row, bound_pos; BCK(bound_row.alloc(bound_cap)); BCK(bound_pos.alloc(bound_cap));
-	Dev<unsigned long long> scal; BCK(scal.alloc(32)); BCK(cudaMemset(scal.p, 0, 32 * 8));   // [0..15] hist, [16] n_bound, [17] zoff, [18] select count
-	Dev<uint64_t> d_frag_start; Dev<uint32_t> d_frag_seq;
+	DBuf<uint64_t> bound_row, bound_pos; BCK(bound_row.alloc(bound_cap)); BCK(bound_pos.alloc(bound_cap));
+	DBuf<unsigned long long> scal; BCK(scal.alloc(32)); BCK(cudaMemset(scal.p, 0, 32 * 8));   // [0..15] hist, [16] n_bound, [17] zoff, [18] select count
+	DBuf<uint64_t> d_frag_start; DBuf<uint32_t> d_frag_seq;
 	BCK(d_frag_start.alloc(m.frag_start.size())); BCK(d_frag_seq.alloc(m.frag_seq.size()));
 	BCK(cudaMemcpy(d_frag_start.p, m.frag_start.data(), m.frag_start.size() * 8, cudaMemcpyHostToDevice));
 	BCK(cudaMemcpy(d_frag_seq.p, m.frag_seq.data(), m.frag_seq.size() * 4, cudaMemcpyHostToDevice));
@@ -499,9 +493,9 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 	const uint32_t cap = (uint32_t)maxb + 1;
 
 	// ---- per-bucket workspace
-	Dev<uint64_t> pos, pos_alt, key, key_alt, key2, key2_alt, pos_tmp;
-	Dev<uint8_t> head, tied, newhead;
-	Dev<uint32_t> headidx, gidfull, idx, perm, perm_alt, gid, gid_s, gid_s_alt;
+	DBuf<uint64_t> pos, pos_alt, key, key_alt, key2, key2_alt, pos_tmp;
+	DBuf<uint8_t> head, tied, newhead;
+	DBuf<uint32_t> headidx, gidfull, idx, perm, perm_alt, gid, gid_s, gid_s_alt;
 	BCK(pos.alloc(cap)); BCK(pos_alt.alloc(cap)); BCK(key.alloc(cap)); BCK(key_alt.alloc(cap));
 	BCK(head.alloc(cap)); BCK(tied.alloc(cap)); BCK(headidx.alloc(cap)); BCK(gidfull.alloc(cap)); BCK(idx.alloc(cap));
 	size_t tmp_bytes = 0, tb = 0;
@@ -519,7 +513,7 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 		cub::DeviceSelect::Flagged(nullptr, tb, c32, tied.p, idx.p, (unsigned long long*)scal.p, (int)cap); tmp_bytes = std::max(tmp_bytes, tb);
 		cub::DeviceScan::InclusiveScan(nullptr, tb, headidx.p, gidfull.p, cub::Max(), (int)cap); tmp_bytes = std::max(tmp_bytes, tb);
 	}
-	Dev<uint8_t> tmp; BCK(tmp.alloc(tmp_bytes + 256));
+	DBuf<uint8_t> tmp; BCK(tmp.alloc(tmp_bytes + 256));
 	bool round_ws = false;       // refinement buffers are allocated on first use (sized by the first tie count)
 	uint32_t round_cap = 0;
 
@@ -622,7 +616,7 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 	// ---- sides: per-side counts -> exclusive occ, '$' not counted as A
 	unsigned long long zoff = 0, nbound = 0;
 	BCK(cudaMemcpy(&nbound, scal.p + 16, 8, cudaMemcpyDeviceToHost)); BCK(cudaMemcpy(&zoff, scal.p + 17, 8, cudaMemcpyDeviceToHost));
-	Dev<uint64_t> cnt; BCK(cnt.alloc(num_sides * 4));
+	DBuf<uint64_t> cnt; BCK(cnt.alloc(num_sides * 4));
 	k_side_counts<<<(unsigned)((num_sides + 255) / 256), 256>>>(bwt.p, num_sides, cnt.p);
 	std::vector<uint64_t> hcnt(num_sides * 4);
 	BCK(cudaMemcpy(hcnt.data(), cnt.p, hcnt.size() * 8, cudaMemcpyDeviceToHost));
@@ -633,7 +627,7 @@ extern "C" int cfb_build_index(const cfb_build_opts* o) {
 	// padding rows past the end of the BWT were counted as A in the last side only: they do not affect any stored occ
 	tot[0] -= (num_sides * 384 - bwt_len);
 	BCK(cudaMemcpy(cnt.p, hcnt.data(), hcnt.size() * 8, cudaMemcpyHostToDevice));
-	Dev<uint32_t> sides; BCK(sides.alloc(num_sides * 32));
+	DBuf<uint32_t> sides; BCK(sides.alloc(num_sides * 32));
 	k_assemble_sides<<<(unsigned)((num_sides * 32 + 255) / 256), 256>>>(bwt.p, cnt.p, num_sides, sides.p);
 	BCK(cudaDeviceSynchronize());
 
@@ -759,7 +753,7 @@ extern "C" int cfb_synth_reads(const cfb_build_opts* o, uint64_t n, uint32_t rdl
 	BCK(cudaSetDevice(o->device));
 	SynthSpec sp; sp.genera = o->synth_genera; sp.species = o->synth_species; sp.len = o->synth_len; sp.seed = o->synth_seed;
 	sp.div_q32 = (uint32_t)std::min(4294967295.0, o->synth_div * 4294967296.0);
-	Dev<uint8_t> d; BCK(d.alloc(n * rdlen));
+	DBuf<uint8_t> d; BCK(d.alloc(n * rdlen));
 	k_synth_reads<<<(unsigned)((n + 127) / 128), 128>>>(sp, n, rdlen, read_seed, d.p);
 	BCK(cudaMemcpy(out_codes, d.p, n * rdlen, cudaMemcpyDeviceToHost));
 	return CFB_OK;
@@ -810,7 +804,7 @@ extern "C" int cfb_synth_reads_ex(const cfb_build_opts* o, const cfb_synth_read_
 	SynthSpec sp; sp.genera = o->synth_genera; sp.species = o->synth_species; sp.len = o->synth_len; sp.seed = o->synth_seed;
 	sp.div_q32 = (uint32_t)std::min(4294967295.0, o->synth_div * 4294967296.0);
 	const uint64_t mates = ro->paired ? 2 : 1;
-	Dev<uint8_t> d; BCK(d.alloc(n * mates * ro->len_hi)); Dev<uint32_t> dl; BCK(dl.alloc(n * mates));
+	DBuf<uint8_t> d; BCK(d.alloc(n * mates * ro->len_hi)); DBuf<uint32_t> dl; BCK(dl.alloc(n * mates));
 	k_synth_reads_ex<<<(unsigned)((n + 127) / 128), 128>>>(sp, *ro, n, read_seed, d.p, dl.p);
 	BCK(cudaMemcpy(out_codes, d.p, n * mates * ro->len_hi, cudaMemcpyDeviceToHost));
 	BCK(cudaMemcpy(out_lens, dl.p, n * mates * 4, cudaMemcpyDeviceToHost));

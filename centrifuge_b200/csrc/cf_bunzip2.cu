@@ -21,6 +21,7 @@
 // and the staging buffer, never on the file size or on how far a block expands.
 #include "../../include/cfb200.h"
 #include "cf_bzip2.h"
+#include "cf_buf.cuh"
 
 #include <cuda_runtime.h>
 
@@ -28,6 +29,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -275,19 +277,6 @@ __global__ void k_bz_crc(const BlkInfo* blk, const uint32_t* win, int nw, const 
 	bcrc[y] = ~reg;
 }
 
-template <class T> struct DBuf {
-	T* p = nullptr; size_t cap = 0;
-	cudaError_t ensure(size_t n) {
-		if(n <= cap) return cudaSuccess;
-		if(p) cudaFree(p);
-		p = nullptr; cap = 0;
-		const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-		if(e == cudaSuccess) cap = n;
-		return e;
-	}
-	void release() { if(p) cudaFree(p); p = nullptr; cap = 0; }
-};
-
 enum Phase { PH_HEADER = 0, PH_BLOCKS = 1, PH_GARBAGE = 2 };
 enum ItemKind { IT_BLOCK = 0, IT_EOS = 1 };
 struct Item { int kind; uint32_t a; uint32_t crc; uint32_t total; };
@@ -295,13 +284,13 @@ struct Item { int kind; uint32_t a; uint32_t crc; uint32_t total; };
 }  // namespace
 
 struct cfb_bunzip2 {
-	int device = 0; cudaStream_t st = nullptr;
+	int device = 0; Stream st;
 	uint64_t span = 64ull << 20;    // compressed bytes scanned per pass
 	uint32_t slots = 512;           // blocks decoded per pass
 	DBuf<uint8_t> d_in, d_L, d_out, d_rend, d_segr; DBuf<uint64_t> d_cand, d_bits, d_woff;
 	DBuf<uint32_t> d_count, d_hist, d_segcnt, d_tt, d_rnext, d_rdist, d_rrank, d_rlen, d_segoff, d_segcrc, d_win, d_bcrc;
 	DBuf<cbz::BlockResult> d_res; DBuf<BlkInfo> d_blk;
-	uint8_t* h_out = nullptr;       // pinned staging, kStage bytes
+	HBuf<uint8_t> h_out;            // pinned staging, kStage bytes
 	// stream state: bit offset relative to the first byte the next call's input starts with
 	int phase = PH_HEADER; uint64_t bit = 0; int level = 9; uint32_t scrc = 0; uint64_t headers = 0;
 	std::vector<Item> items; size_t next_item = 0;      // the decoded pass, delivered in order
@@ -309,6 +298,7 @@ struct cfb_bunzip2 {
 	uint64_t streams = 0, in_total = 0, out_total = 0, blocks = 0, rejected = 0, trailing = 0;
 	size_t pend_lo = 0, pend_hi = 0;
 	int err = 0; std::string err_msg;
+	~cfb_bunzip2() { cudaSetDevice(device); if(st) cudaStreamSynchronize(st); }
 };
 
 namespace {
@@ -335,7 +325,7 @@ int bz_pass(cfb_bunzip2* g, const uint8_t* in0, uint64_t n0, bool is_last, bool*
 	std::vector<cbz::BlockResult> res;
 	uint64_t scan_hi = std::min(up, g->span) * 8;
 	if(scan_hi > b) {
-		BZ_CK(g->d_in.ensure(g->span + kLook + 16)); BZ_CK(g->d_cand.ensure(kCandCap)); BZ_CK(g->d_count.ensure(1));
+		BZ_CK(g->d_in.ensure_exact(g->span + kLook + 16)); BZ_CK(g->d_cand.ensure_exact(kCandCap)); BZ_CK(g->d_count.ensure_exact(1));
 		BZ_CK(cudaMemcpyAsync(g->d_in.p, in, up, cudaMemcpyHostToDevice, g->st));
 		uint32_t count = 0;
 		for(;;) {
@@ -358,7 +348,7 @@ int bz_pass(cfb_bunzip2* g, const uint8_t* in0, uint64_t n0, bool is_last, bool*
 		const uint32_t k = (uint32_t)std::min<size_t>(cands.size(), g->slots);
 		if(k) {
 			res.resize(k);
-			BZ_CK(g->d_bits.ensure(k)); BZ_CK(g->d_L.ensure((size_t)k * BLOCK_MAX)); BZ_CK(g->d_hist.ensure((size_t)k * 256)); BZ_CK(g->d_res.ensure(k));
+			BZ_CK(g->d_bits.ensure_exact(k)); BZ_CK(g->d_L.ensure_exact((size_t)k * BLOCK_MAX)); BZ_CK(g->d_hist.ensure_exact((size_t)k * 256)); BZ_CK(g->d_res.ensure_exact(k));
 			BZ_CK(cudaMemcpyAsync(g->d_bits.p, cands.data(), k * 8ull, cudaMemcpyHostToDevice, g->st));
 			k_bz_decode<<<k, 1, 0, g->st>>>(g->d_in.p, up, g->d_bits.p, g->d_L.p, g->d_hist.p, g->d_res.p);
 			BZ_CK(cudaGetLastError());
@@ -417,10 +407,10 @@ int bz_pass(cfb_bunzip2* g, const uint8_t* in0, uint64_t n0, bool is_last, bool*
 	if(acc.empty()) return 0;
 	// 4-5: inverse BWT and RLE1 counts of the accepted blocks
 	const int na = (int)acc.size();
-	BZ_CK(g->d_blk.ensure(na)); BZ_CK(g->d_segcnt.ensure((size_t)na * kNSeg * 256)); BZ_CK(g->d_tt.ensure((size_t)na * BLOCK_MAX));
-	BZ_CK(g->d_rnext.ensure((size_t)na * kNR)); BZ_CK(g->d_rdist.ensure((size_t)na * kNR)); BZ_CK(g->d_rrank.ensure((size_t)na * kNR));
-	BZ_CK(g->d_rlen.ensure((size_t)na * kNSeg * 5)); BZ_CK(g->d_rend.ensure((size_t)na * kNSeg * 5));
-	BZ_CK(g->d_segr.ensure((size_t)na * kNSeg)); BZ_CK(g->d_segoff.ensure((size_t)na * kNSeg)); BZ_CK(g->d_segcrc.ensure((size_t)na * kNSeg));
+	BZ_CK(g->d_blk.ensure_exact(na)); BZ_CK(g->d_segcnt.ensure_exact((size_t)na * kNSeg * 256)); BZ_CK(g->d_tt.ensure_exact((size_t)na * BLOCK_MAX));
+	BZ_CK(g->d_rnext.ensure_exact((size_t)na * kNR)); BZ_CK(g->d_rdist.ensure_exact((size_t)na * kNR)); BZ_CK(g->d_rrank.ensure_exact((size_t)na * kNR));
+	BZ_CK(g->d_rlen.ensure_exact((size_t)na * kNSeg * 5)); BZ_CK(g->d_rend.ensure_exact((size_t)na * kNSeg * 5));
+	BZ_CK(g->d_segr.ensure_exact((size_t)na * kNSeg)); BZ_CK(g->d_segoff.ensure_exact((size_t)na * kNSeg)); BZ_CK(g->d_segcrc.ensure_exact((size_t)na * kNSeg));
 	BZ_CK(cudaMemcpyAsync(g->d_blk.p, acc.data(), na * sizeof(BlkInfo), cudaMemcpyHostToDevice, g->st));
 	BZ_CK(cudaMemsetAsync(g->d_rrank.p, 0xff, (size_t)na * kNR * 4, g->st));
 	const dim3 gseg((kNSeg + 7) / 8, na), grul((kNR + 127) / 128, na), grle((kNSeg + 63) / 64, na);
@@ -461,15 +451,15 @@ int bz_deliver(cfb_bunzip2* g) {
 	const int nw = (int)win.size();
 	std::vector<uint32_t> got(nw);
 	if(nw) {
-		BZ_CK(g->d_out.ensure(kStage)); BZ_CK(g->d_win.ensure(nw)); BZ_CK(g->d_woff.ensure(nw)); BZ_CK(g->d_bcrc.ensure(nw));
-		if(!g->h_out) BZ_CK(cudaHostAlloc((void**)&g->h_out, kStage, cudaHostAllocPortable));
+		BZ_CK(g->d_out.ensure_exact(kStage)); BZ_CK(g->d_win.ensure_exact(nw)); BZ_CK(g->d_woff.ensure_exact(nw)); BZ_CK(g->d_bcrc.ensure_exact(nw));
+		BZ_CK(g->h_out.ensure_exact(kStage));
 		BZ_CK(cudaMemcpyAsync(g->d_win.p, win.data(), nw * 4ull, cudaMemcpyHostToDevice, g->st));
 		BZ_CK(cudaMemcpyAsync(g->d_woff.p, off.data(), nw * 8ull, cudaMemcpyHostToDevice, g->st));
 		k_bz_expand<<<dim3((kNSeg + 63) / 64, nw), 64, 0, g->st>>>(g->d_L.p, g->d_blk.p, g->d_win.p, g->d_woff.p, g->d_segr.p, g->d_segoff.p, g->d_out.p, g->d_segcrc.p);
 		k_bz_crc<<<(nw + 31) / 32, 32, 0, g->st>>>(g->d_blk.p, g->d_win.p, nw, g->d_segoff.p, g->d_segcrc.p, g->d_bcrc.p);
 		BZ_CK(cudaGetLastError());
 		BZ_CK(cudaMemcpyAsync(got.data(), g->d_bcrc.p, nw * 4ull, cudaMemcpyDeviceToHost, g->st));
-		BZ_CK(cudaMemcpyAsync(g->h_out, g->d_out.p, total, cudaMemcpyDeviceToHost, g->st));
+		BZ_CK(cudaMemcpyAsync(g->h_out.p, g->d_out.p, total, cudaMemcpyDeviceToHost, g->st));
 		BZ_CK(cudaStreamSynchronize(g->st));
 	}
 	for(int i = 0; g->next_item < end; g->next_item++) {
@@ -498,27 +488,16 @@ extern "C" int cfb_bunzip2_create(int device, uint32_t pass_kb, cfb_bunzip2** ou
 	if(pass_kb == 0) { const char* e = getenv("CFB_BZ2_PASS_KB"); pass_kb = e ? (uint32_t)strtoul(e, NULL, 10) : 65536; }
 	if(pass_kb < 1 || pass_kb > (1u << 20)) return cfb_fail_msg(CFB_EINVAL, "bzip2 pass size must be 1 to 1048576 KB");
 	if(cudaSetDevice(device) != cudaSuccess) return cfb_fail_msg(CFB_ECUDA, "cudaSetDevice failed");
-	cfb_bunzip2* g = new cfb_bunzip2();
+	std::unique_ptr<cfb_bunzip2> g(new cfb_bunzip2());
 	g->device = device; g->span = (uint64_t)pass_kb << 10;
 	// a level-9 block of FASTQ compresses to about 230 KB: a slot per 128 KB of span, at most 512 (about 2.5 GB)
 	g->slots = (uint32_t)std::min<uint64_t>(512, std::max<uint64_t>(4, g->span >> 17));
-	if(cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) != cudaSuccess) { delete g; return cfb_fail_msg(CFB_ECUDA, "cudaStreamCreate failed"); }
-	*out = g;
+	if(g->st.create() != cudaSuccess) return cfb_fail_msg(CFB_ECUDA, "cudaStreamCreate failed");
+	*out = g.release();
 	return CFB_OK;
 }
 
-extern "C" void cfb_bunzip2_destroy(cfb_bunzip2* g) {
-	if(!g) return;
-	cudaSetDevice(g->device);
-	if(g->st) cudaStreamSynchronize(g->st);
-	g->d_in.release(); g->d_L.release(); g->d_out.release(); g->d_rend.release(); g->d_segr.release(); g->d_cand.release(); g->d_bits.release();
-	g->d_woff.release(); g->d_count.release(); g->d_hist.release(); g->d_segcnt.release(); g->d_tt.release(); g->d_rnext.release();
-	g->d_rdist.release(); g->d_rrank.release(); g->d_rlen.release(); g->d_segoff.release(); g->d_segcrc.release(); g->d_win.release();
-	g->d_bcrc.release(); g->d_res.release(); g->d_blk.release();
-	if(g->h_out) cudaFreeHost(g->h_out);
-	if(g->st) cudaStreamDestroy(g->st);
-	delete g;
-}
+extern "C" void cfb_bunzip2_destroy(cfb_bunzip2* g) { delete g; }
 
 extern "C" int cfb_bunzip2_run(cfb_bunzip2* g, const void* in_, uint64_t n_in, int in_is_last, void* out, uint64_t out_cap,
                                uint64_t* n_out, uint64_t* n_consumed) {
@@ -551,7 +530,7 @@ extern "C" int cfb_bunzip2_run(cfb_bunzip2* g, const void* in_, uint64_t n_in, i
 	g->in_total += pos;
 	*n_consumed = pos;
 	const uint64_t give = std::min<uint64_t>(out_cap, g->pend_hi - g->pend_lo);
-	if(give) { if(out) memcpy(out, g->h_out + g->pend_lo, give); g->pend_lo += give; }
+	if(give) { if(out) memcpy(out, g->h_out.p + g->pend_lo, give); g->pend_lo += give; }
 	*n_out = give;
 	return CFB_OK;
 }

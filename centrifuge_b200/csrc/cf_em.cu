@@ -11,6 +11,7 @@
 // and every multiply/add/divide is issued through the _rn intrinsics so that nothing is contracted into an FMA.
 // The host (cf_host.cpp) flattens `observed` and computes the start vector; only the iteration runs here.
 #include "../../include/cfb200.h"
+#include "cf_buf.cuh"
 
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -111,8 +112,7 @@ extern "C" const char* cfb_em_last_error(void) { return g_em_err; }
 extern "C" int cfb_em_abundance(int device, uint64_t n, uint64_t K, const uint64_t* count, const uint64_t* key_off, const uint32_t* target,
                                 const uint64_t* len, double* p, uint64_t* iters, double* last_diff) {
 	if(!count || !key_off || !target || !len || !p || !iters || !last_diff || n == 0 || n >= (1ull << 32) || K >= (1ull << 32)) return CFB_EINVAL;
-	#define EK(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { snprintf(g_em_err, sizeof g_em_err, "%s failed: %s", #call, cudaGetErrorString(e_)); for(size_t q_ = 0; q_ < bufs.size(); q_++) cudaFree(bufs[q_]); return CFB_ECUDA; } } while(0)
-	std::vector<void*> bufs;
+	#define EK(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { snprintf(g_em_err, sizeof g_em_err, "%s failed: %s", #call, cudaGetErrorString(e_)); return CFB_ECUDA; } } while(0)
 	EK(cudaSetDevice(device));
 	const uint64_t T = key_off[K];
 	// incidence lists: species j <- the keys that reach it, in (key, position) order (counting sort keeps it)
@@ -121,25 +121,24 @@ extern "C" int cfb_em_abundance(int device, uint64_t n, uint64_t K, const uint64
 	for(uint64_t j = 0; j < n; j++) inc_off[j + 1] += inc_off[j];
 	{ std::vector<uint64_t> fill(inc_off.begin(), inc_off.end() - 1);
 	  for(uint64_t k = 0; k < K; k++) for(uint64_t t = key_off[k]; t < key_off[k + 1]; t++) inc_key[fill[target[t]]++] = (uint32_t)k; }
-	auto up = [&](const void* src, size_t bytes, void** dst) -> cudaError_t {
-		cudaError_t e = cudaMalloc(dst, bytes ? bytes : 8); if(e != cudaSuccess) return e;
-		bufs.push_back(*dst);
-		return bytes ? cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice) : cudaSuccess;
+	auto up = [&](const void* src, size_t bytes, DBuf<uint8_t>& dst) -> cudaError_t {
+		cudaError_t e = dst.alloc(bytes ? bytes : 8); if(e != cudaSuccess) return e;
+		return bytes ? cudaMemcpy(dst.p, src, bytes, cudaMemcpyHostToDevice) : cudaSuccess;
 	};
 	EmArgs a; a.n = n; a.K = K;
-	void *d_count, *d_koff, *d_tgt, *d_ioff, *d_ikey, *d_len, *d_psum, *d_scal, *d_p, *d_pn, *d_pn2, *d_pr, *d_pv, *d_q, *d_q2;
-	EK(up(count, K * 8, &d_count)); EK(up(key_off, (K + 1) * 8, &d_koff)); EK(up(target, T * 4, &d_tgt));
-	EK(up(inc_off.data(), (n + 1) * 8, &d_ioff)); EK(up(inc_key.data(), T * 4, &d_ikey)); EK(up(len, n * 8, &d_len));
-	EK(cudaMalloc(&d_psum, (K + 1) * 8)); bufs.push_back(d_psum);
-	EK(cudaMalloc(&d_scal, 8 * 8)); bufs.push_back(d_scal); EK(cudaMemset(d_scal, 0, 64));
-	EK(up(p, n * 8, &d_p));
-	EK(cudaMalloc(&d_pn, n * 8)); bufs.push_back(d_pn); EK(cudaMalloc(&d_pn2, n * 8)); bufs.push_back(d_pn2);
-	EK(cudaMalloc(&d_pr, n * 8)); bufs.push_back(d_pr); EK(cudaMalloc(&d_pv, n * 8)); bufs.push_back(d_pv);
-	EK(cudaMalloc(&d_q, n * 8)); bufs.push_back(d_q); EK(cudaMalloc(&d_q2, n * 8)); bufs.push_back(d_q2);
-	a.count = (const uint64_t*)d_count; a.key_off = (const uint64_t*)d_koff; a.target = (const uint32_t*)d_tgt;
-	a.inc_off = (const uint64_t*)d_ioff; a.inc_key = (const uint32_t*)d_ikey; a.len = (const uint64_t*)d_len;
-	a.psum = (double*)d_psum; a.scal = (double*)d_scal;
-	double *P = (double*)d_p, *PN = (double*)d_pn, *PN2 = (double*)d_pn2, *PR = (double*)d_pr, *PV = (double*)d_pv, *Q = (double*)d_q, *Q2 = (double*)d_q2;
+	DBuf<uint8_t> d_count, d_koff, d_tgt, d_ioff, d_ikey, d_len, d_p; DBuf<double> d_psum, d_scal, d_pn, d_pn2, d_pr, d_pv, d_q, d_q2;
+	EK(up(count, K * 8, d_count)); EK(up(key_off, (K + 1) * 8, d_koff)); EK(up(target, T * 4, d_tgt));
+	EK(up(inc_off.data(), (n + 1) * 8, d_ioff)); EK(up(inc_key.data(), T * 4, d_ikey)); EK(up(len, n * 8, d_len));
+	EK(d_psum.alloc(K + 1));
+	EK(d_scal.alloc(8)); EK(cudaMemset(d_scal.p, 0, 64));
+	EK(up(p, n * 8, d_p));
+	EK(d_pn.alloc(n)); EK(d_pn2.alloc(n));
+	EK(d_pr.alloc(n)); EK(d_pv.alloc(n));
+	EK(d_q.alloc(n)); EK(d_q2.alloc(n));
+	a.count = (const uint64_t*)d_count.p; a.key_off = (const uint64_t*)d_koff.p; a.target = (const uint32_t*)d_tgt.p;
+	a.inc_off = (const uint64_t*)d_ioff.p; a.inc_key = (const uint32_t*)d_ikey.p; a.len = (const uint64_t*)d_len.p;
+	a.psum = d_psum.p; a.scal = d_scal.p;
+	double *P = (double*)d_p.p, *PN = d_pn.p, *PN2 = d_pn2.p, *PR = d_pr.p, *PV = d_pv.p, *Q = d_q.p, *Q2 = d_q2.p;
 	const unsigned bk = (unsigned)((K + 255) / 256), bn = (unsigned)((n + 255) / 256);
 	auto em_step = [&](const double* src, double* dst, int guarded) {
 		if(bk) k_em_psum<<<bk, 256>>>(a, src, guarded);
@@ -158,14 +157,13 @@ extern "C" int cfb_em_abundance(int device, uint64_t n, uint64_t K, const uint64
 		em_step(PN2, PN, 1);
 		k_em_absdiff<<<bn, 256>>>(a, P, PN, Q);
 		k_em_converged<<<1, 1>>>(a, Q);
-		EK(cudaMemcpy(sc, d_scal, 64, cudaMemcpyDeviceToHost));
+		EK(cudaMemcpy(sc, d_scal.p, 64, cudaMemcpyDeviceToHost));
 		if(sc[5] != 0.0) break;
 		if(++it >= 10000) break;
 		double* tmp = P; P = PN; PN = tmp;                      // p = pn
 	}
 	EK(cudaMemcpy(p, P, n * 8, cudaMemcpyDeviceToHost));
 	*iters = it; *last_diff = sc[3];
-	for(size_t q = 0; q < bufs.size(); q++) cudaFree(bufs[q]);
 	#undef EK
 	return CFB_OK;
 }

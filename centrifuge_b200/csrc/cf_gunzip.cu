@@ -11,6 +11,7 @@
 // host.  Memory depends on the chunk size (the span is kMaxChunks chunks), never on the file size.
 #include "../../include/cfb200.h"
 #include "cf_inflate.h"
+#include "cf_buf.cuh"
 
 #include <cuda_runtime.h>
 
@@ -18,6 +19,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -147,37 +149,12 @@ uint32_t crc32_host(uint32_t c, const uint8_t* p, size_t n) {       // member he
 	return ~c;
 }
 
-template <class T> struct DBuf {
-	T* p = nullptr; size_t cap = 0;
-	cudaError_t ensure(size_t n) {
-		if(n <= cap) return cudaSuccess;
-		if(p) cudaFree(p);
-		p = nullptr; cap = 0;
-		const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
-		if(e == cudaSuccess) cap = n;
-		return e;
-	}
-	void release() { if(p) cudaFree(p); p = nullptr; cap = 0; }
-};
-template <class T> struct HBuf {
-	T* p = nullptr; size_t cap = 0;
-	cudaError_t ensure(size_t n) {
-		if(n <= cap) return cudaSuccess;
-		if(p) cudaFreeHost(p);
-		p = nullptr; cap = 0;
-		const cudaError_t e = cudaHostAlloc((void**)&p, n * sizeof(T), cudaHostAllocPortable);
-		if(e == cudaSuccess) cap = n;
-		return e;
-	}
-	void release() { if(p) cudaFreeHost(p); p = nullptr; cap = 0; }
-};
-
 enum Phase { PH_HEADER = 0, PH_DEFLATE = 1, PH_TRAILER = 2 };
 
 }  // namespace
 
 struct cfb_gunzip {
-	int device = 0; cudaStream_t st = nullptr;
+	int device = 0; Stream st;
 	uint64_t chunk = 64 << 10;      // compressed bytes per chunk
 	uint32_t cap = 0;               // symbols per chunk
 	DBuf<uint8_t> d_in, d_prev, d_win, d_out;      // d_prev: the window carried from the previous pass
@@ -190,6 +167,7 @@ struct cfb_gunzip {
 	uint64_t in_total = 0, out_total = 0, members = 0, chunks = 0, redone = 0;
 	size_t pend_lo = 0, pend_hi = 0;
 	int err = 0; std::string err_msg;
+	~cfb_gunzip() { cudaSetDevice(device); if(st) cudaStreamSynchronize(st); }
 };
 
 namespace {
@@ -251,9 +229,9 @@ int gz_pass(cfb_gunzip* g, const uint8_t* in0, uint64_t n0, bool is_last, bool* 
 	for(int c = 0; c < nch; c++) nom[c] = bit + (uint64_t)c * cb;
 	nom[nch] = pass_stop;
 	auto stop_of = [&](int c) { return c + 1 < nch ? nom[c + 1] : pass_stop; };
-	GZ_CK(g->d_in.ensure(up + 8)); GZ_CK(g->d_sym.ensure((size_t)nch * g->cap)); GZ_CK(g->d_ci.ensure(nch)); GZ_CK(g->d_res.ensure(nch));
-	GZ_CK(g->d_nom.ensure(nch + 1)); GZ_CK(g->d_found.ensure(nch)); GZ_CK(g->d_win.ensure((size_t)(nch + 1) * WIN));
-	GZ_CK(g->d_prev.ensure(WIN));
+	GZ_CK(g->d_in.ensure_exact(up + 8)); GZ_CK(g->d_sym.ensure_exact((size_t)nch * g->cap)); GZ_CK(g->d_ci.ensure_exact(nch)); GZ_CK(g->d_res.ensure_exact(nch));
+	GZ_CK(g->d_nom.ensure_exact(nch + 1)); GZ_CK(g->d_found.ensure_exact(nch)); GZ_CK(g->d_win.ensure_exact((size_t)(nch + 1) * WIN));
+	GZ_CK(g->d_prev.ensure_exact(WIN));
 	GZ_CK(cudaMemcpyAsync(g->d_win.p, g->d_prev.p, WIN, cudaMemcpyDeviceToDevice, g->st));
 	GZ_CK(cudaMemcpyAsync(g->d_in.p, in, up, cudaMemcpyHostToDevice, g->st));
 	if(nch > 1) {
@@ -310,8 +288,8 @@ int gz_pass(cfb_gunzip* g, const uint8_t* in0, uint64_t n0, bool is_last, bool* 
 	const uint64_t total = off[k];
 	if(total) {
 		const uint64_t npieces = (total + kCrcPiece - 1) / kCrcPiece;
-		GZ_CK(g->d_out.ensure(total + 8)); GZ_CK(g->h_out.ensure(total)); GZ_CK(g->d_crc.ensure(npieces)); GZ_CK(g->h_crc.ensure(npieces));
-		GZ_CK(g->d_nsym.ensure(k)); GZ_CK(g->d_minm.ensure(k)); GZ_CK(g->d_off.ensure(k + 1)); GZ_CK(g->d_err.ensure(1));
+		GZ_CK(g->d_out.ensure_exact(total + 8)); GZ_CK(g->h_out.ensure_exact(total)); GZ_CK(g->d_crc.ensure_exact(npieces)); GZ_CK(g->h_crc.ensure_exact(npieces));
+		GZ_CK(g->d_nsym.ensure_exact(k)); GZ_CK(g->d_minm.ensure_exact(k)); GZ_CK(g->d_off.ensure_exact(k + 1)); GZ_CK(g->d_err.ensure_exact(1));
 		GZ_CK(cudaMemcpyAsync(g->d_nsym.p, nsym.data(), k * 4, cudaMemcpyHostToDevice, g->st));
 		GZ_CK(cudaMemcpyAsync(g->d_minm.p, minm.data(), k * 4, cudaMemcpyHostToDevice, g->st));
 		GZ_CK(cudaMemcpyAsync(g->d_off.p, off.data(), (k + 1) * 8, cudaMemcpyHostToDevice, g->st));
@@ -354,26 +332,17 @@ extern "C" int cfb_gunzip_create(int device, uint32_t chunk_kb, cfb_gunzip** out
 	if(chunk_kb == 0) { const char* e = getenv("CFB_GZ_CHUNK_KB"); chunk_kb = e ? (uint32_t)strtoul(e, NULL, 10) : 64; }
 	if(chunk_kb < 1 || chunk_kb > 4096) return cfb_fail_msg(CFB_EINVAL, "gzip chunk size must be 1 to 4096 KB");
 	if(cudaSetDevice(device) != cudaSuccess) return cfb_fail_msg(CFB_ECUDA, "cudaSetDevice failed");
-	cfb_gunzip* g = new cfb_gunzip();
+	std::unique_ptr<cfb_gunzip> g(new cfb_gunzip());
 	g->device = device; g->chunk = (uint64_t)chunk_kb << 10;
 	// FASTQ compresses 3-6x, and a chunk decodes one block past its end: a chunk that expands further than this stops
 	// early and its successor is re-decoded, which serialises the pass
 	g->cap = (uint32_t)(12 * g->chunk + 131072 + 258);
-	if(cudaStreamCreateWithFlags(&g->st, cudaStreamNonBlocking) != cudaSuccess) { delete g; return cfb_fail_msg(CFB_ECUDA, "cudaStreamCreate failed"); }
-	*out = g;
+	if(g->st.create() != cudaSuccess) return cfb_fail_msg(CFB_ECUDA, "cudaStreamCreate failed");
+	*out = g.release();
 	return CFB_OK;
 }
 
-extern "C" void cfb_gunzip_destroy(cfb_gunzip* g) {
-	if(!g) return;
-	cudaSetDevice(g->device);
-	if(g->st) cudaStreamSynchronize(g->st);
-	g->d_in.release(); g->d_prev.release(); g->d_win.release(); g->d_out.release(); g->d_sym.release(); g->d_ci.release(); g->d_res.release();
-	g->d_nom.release(); g->d_found.release(); g->d_off.release(); g->d_nsym.release(); g->d_minm.release(); g->d_crc.release(); g->d_err.release();
-	g->h_out.release(); g->h_crc.release();
-	if(g->st) cudaStreamDestroy(g->st);
-	delete g;
-}
+extern "C" void cfb_gunzip_destroy(cfb_gunzip* g) { delete g; }
 
 extern "C" int cfb_gunzip_run(cfb_gunzip* g, const void* in_, uint64_t n_in, int in_is_last, void* out, uint64_t out_cap,
                               uint64_t* n_out, uint64_t* n_consumed) {
@@ -442,7 +411,7 @@ extern "C" int cfb_gunzip_set_state(cfb_gunzip* g, const cfb_gunzip_state* s) {
 	if(s->phase < PH_HEADER || s->phase > PH_TRAILER || s->win_len > (uint32_t)WIN || (s->phase != PH_DEFLATE && (s->bit || s->hdr_bit != NONE)))
 		return cfb_fail_msg(CFB_EINVAL, "cfb_gunzip_set_state: invalid state");
 	if(cudaSetDevice(g->device) != cudaSuccess) return cfb_fail_msg(CFB_ECUDA, "cudaSetDevice failed");
-	if(g->d_prev.ensure(WIN) != cudaSuccess || cudaMemcpy(g->d_prev.p, s->window, WIN, cudaMemcpyHostToDevice) != cudaSuccess)
+	if(g->d_prev.ensure_exact(WIN) != cudaSuccess || cudaMemcpy(g->d_prev.p, s->window, WIN, cudaMemcpyHostToDevice) != cudaSuccess)
 		return cfb_fail_msg(CFB_ECUDA, "cfb_gunzip_set_state: window copy failed");
 	g->in_total = s->in_offset; g->out_total = s->out_offset; g->bit = s->bit; g->hdr = s->hdr_bit; g->msize = s->member_bytes;
 	g->crc = s->crc; g->win_len = s->win_len; g->phase = s->phase; g->members = s->members;

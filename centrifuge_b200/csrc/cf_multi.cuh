@@ -97,17 +97,10 @@ bool nccl_load() {
 }  // namespace
 #define NK(call) do { ncclResult_t r_ = (call); if(r_ != ncclSuccess) return fail(CFB_ECUDA, "%s failed: %s", #call, g_nccl.GetErrorString(r_)); } while(0)
 
-static void comm_release(cfb_ctx* c) {
-	if(!c) return;
-	if(c->comm && g_nccl.lib) g_nccl.CommDestroy((ncclComm_t)c->comm);
-	c->comm = nullptr;
-	if(c->comm_st) cudaStreamDestroy(c->comm_st);
-	c->comm_st = nullptr;
-}
 static int comm_prepare(cfb_ctx* c) {
 	CK(cudaSetDevice(c->ix->device));
 	int rc = counts_init(c); if(rc) return rc;
-	if(!c->comm_st) CK(cudaStreamCreateWithFlags(&c->comm_st, cudaStreamNonBlocking));
+	if(!c->comm_st) CK(c->comm_st.create());
 	return CFB_OK;
 }
 static_assert(sizeof(ncclUniqueId) == CFB_COMM_ID_BYTES, "ncclUniqueId size");
@@ -183,14 +176,14 @@ extern "C" int cfb_comm_info(const cfb_ctx* c, int* rank, int* size, int* nccl_v
 extern "C" int cfb_ctx_requests(cfb_ctx* c, uint64_t out[5]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");
 	CK(cudaSetDevice(c->ix->device));
-	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr.p, sizeof h, cudaMemcpyDeviceToHost));
 	out[0] = h.req_rank16; out[1] = h.req_ftab2; out[2] = h.req_ftabk; out[3] = h.req_walk8; out[4] = h.req_ftabd;
 	return CFB_OK;
 }
 extern "C" int cfb_ctx_request_breakdown(cfb_ctx* c, uint64_t out[8]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");
 	CK(cudaSetDevice(c->ix->device));
-	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr.p, sizeof h, cudaMemcpyDeviceToHost));
 	out[0] = h.r16_w1; out[1] = h.r16_w2_4; out[2] = h.r16_w5;
 	out[3] = h.w8_try_row; out[4] = h.w8_ok_row; out[5] = h.w8_try_range; out[6] = h.w8_ok_range; out[7] = h.w8_ok_w5;
 	return CFB_OK;
@@ -198,7 +191,7 @@ extern "C" int cfb_ctx_request_breakdown(cfb_ctx* c, uint64_t out[8]) {
 extern "C" int cfb_ctx_search_iter_stats(cfb_ctx* c, uint64_t out[8]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");
 	CK(cudaSetDevice(c->ix->device));
-	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr.p, sizeof h, cudaMemcpyDeviceToHost));
 	out[0] = h.it_warp; out[1] = h.it_lane_req; out[2] = h.it_consumers; out[3] = h.it_restarts; out[4] = h.it_task;
 	out[5] = h.clk_head; out[6] = h.clk_wait; out[7] = h.clk_tail;
 	return CFB_OK;
@@ -206,7 +199,7 @@ extern "C" int cfb_ctx_search_iter_stats(cfb_ctx* c, uint64_t out[8]) {
 extern "C" int cfb_ctx_score_stats(cfb_ctx* c, uint64_t out[23]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");
 	CK(cudaSetDevice(c->ix->device));
-	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr.p, sizeof h, cudaMemcpyDeviceToHost));
 	out[0] = h.sc_units; out[1] = h.sc_rows; out[2] = h.sc_nmap; out[3] = h.sc_reduce; out[4] = h.sc_rounds; out[5] = h.sc_warps; out[6] = h.sc_warps_global;
 	for(int i = 0; i < 8; i++) { out[7 + i] = h.sc_rows_hist[i]; out[15 + i] = h.sc_nmap_hist[i]; }
 	return CFB_OK;
@@ -253,16 +246,15 @@ extern "C" int cfb_gather_rate(const cfb_index* ix, int table, uint64_t n_reques
 	const int blocks = ix->sm_count * ctas_per_sm;
 	const uint64_t per_iter = (uint64_t)blocks * threads * ilp;
 	const uint32_t iters = (uint32_t)std::max<uint64_t>(1, n_requests / per_iter);
-	unsigned long long* sink = nullptr; CK(cudaMalloc((void**)&sink, 8));
-	cudaEvent_t e0, e1; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+	DBuf<unsigned long long> sink; CK(sink.alloc(1));
+	Event e0, e1; CK(e0.create()); CK(e1.create());
 	auto launch = [&](uint32_t it) {
-		if(W == 2) { if(ilp == 4) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink); else if(ilp == 2) k_gather_probe<2, 2><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<2, 1><<<blocks, threads>>>(base, n, it, sink); }
-		else { if(ilp == 4) k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink); else if(ilp == 2) k_gather_probe<1, 2><<<blocks, threads>>>(base, n, it, sink); else k_gather_probe<1, 1><<<blocks, threads>>>(base, n, it, sink); }
+		if(W == 2) { if(ilp == 4) k_gather_probe<2, 4><<<blocks, threads>>>(base, n, it, sink.p); else if(ilp == 2) k_gather_probe<2, 2><<<blocks, threads>>>(base, n, it, sink.p); else k_gather_probe<2, 1><<<blocks, threads>>>(base, n, it, sink.p); }
+		else { if(ilp == 4) k_gather_probe<1, 4><<<blocks, threads>>>(base, n, it, sink.p); else if(ilp == 2) k_gather_probe<1, 2><<<blocks, threads>>>(base, n, it, sink.p); else k_gather_probe<1, 1><<<blocks, threads>>>(base, n, it, sink.p); }
 	};
 	launch(std::max<uint32_t>(1, iters / 16)); CK(cudaDeviceSynchronize());      // warm-up
 	CK(cudaEventRecord(e0)); launch(iters); CK(cudaEventRecord(e1)); CK(cudaEventSynchronize(e1));
 	float ms = 0; CK(cudaEventElapsedTime(&ms, e0, e1));
-	cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(sink);
 	CK(cudaGetLastError());
 	*g_requests_per_s = (double)per_iter * iters / ((double)ms * 1e6);
 	if(ms_out) *ms_out = ms;

@@ -471,12 +471,6 @@ struct TextSlot {
 	uint64_t n_rec = 0; int n_mates = 1; cfb_text_opts opt; uint64_t bytes[2] = {0, 0}; bool pending = false;
 	uint64_t spec_tsv = 0, spec_multi = 0;      // bytes / tie-set records already copied home behind the kernels
 	DBuf<uint8_t> d_cols; std::vector<uint8_t> cols;      // column list of the span in flight (device copy of `cols`)
-	void release() {
-		d_cols.release(); cols.clear();
-		for(int m = 0; m < 2; m++) { d_text[m].release(); h_text[m].release(); nl[m].release(); tile_cnt[m].release(); tile_off[m].release(); seedv[m].release(); seq_off[m].release(); qual_off[m].release(); }
-		tbsum.release(); name_off.release(); name_len.release(); id_len.release(); row_bytes.release(); sec.release(); txt_off.release(); sel.release(); num.release();
-		d_tsv.release(); h_tsv.release(); multi.release(); h_multi.release(); sp.release(); tscal.release(); h_tscal.release();
-	}
 };
 struct TextCtx {
 	bool ready = false, names_ready = false;
@@ -488,17 +482,10 @@ struct TextCtx {
 	uint32_t maxlen_hint = 128;
 	double tsv_ratio = 64.0, multi_ratio = 0.05;     // bytes / tie sets per unit seen so far (size the speculative D2H)
 	TextSlot slots[kSlots - 1];
-	void release() {
-		nd_taxid.release(); nd_info.release(); sn_off.release(); sn_blob.release(); rk_off.release(); rk_blob.release();
-		nm_taxid.release(); nm_off.release(); nm_blob.release();
-		for(int i = 0; i < kSlots - 1; i++) slots[i].release();
-	}
 };
 
-static void text_release(cfb_ctx* c) { if(c && c->text) { c->text->release(); delete c->text; c->text = nullptr; } }
-
 static int text_init(cfb_ctx* c) {
-	if(!c->text) c->text = new TextCtx();
+	if(!c->text) c->text.reset(new TextCtx());
 	TextCtx& t = *c->text;
 	if(t.ready) return CFB_OK;
 	const HostIndex& h = c->ix->h;
@@ -547,7 +534,7 @@ extern "C" int cfb_ctx_set_columns(cfb_ctx* c, const char* cols) {
 	ColList l; std::string err;
 	if(!l.parse(cols ? cols : kDefaultCols, err)) return fail(CFB_EINVAL, "%s", err.c_str());
 	if(l.fields.size() > (size_t)kTextMaxCols) return fail(CFB_EINVAL, "the text operator prints at most %d columns", kTextMaxCols);
-	if(!c->text) c->text = new TextCtx();
+	if(!c->text) c->text.reset(new TextCtx());
 	c->text->cols = l.fields;
 	return CFB_OK;
 }
@@ -652,11 +639,6 @@ extern "C" int cfb_text_submit(cfb_ctx* c, int slot, const void* text_a, uint64_
 	t.n_rec = n_rec; t.n_mates = nm; t.opt = *o; t.bytes[0] = bytes_a; t.bytes[1] = text_b ? bytes_b : 0;
 	s.n_units = n_rec; s.bv.n_units = (uint32_t)n_rec; s.bv.n_mates = nm; s.longs.clear(); s.win_first = 0;
 	if(n_rec == 0) { s.pending = true; t.pending = true; return CFB_OK; }
-	auto pinned = [](const void* p) -> bool {
-		cudaPointerAttributes at;
-		if(cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
-		return at.type == cudaMemoryTypeHost;
-	};
 	CK(t.tscal.ensure(8)); CK(t.h_tscal.ensure(8));
 	const void* src[2] = {text_a, text_b};
 	const uint64_t n = n_rec;
@@ -668,7 +650,7 @@ extern "C" int cfb_text_submit(cfb_ctx* c, int slot, const void* text_a, uint64_
 	for(int m = 0; m < nm; m++) {
 		CK(t.d_text[m].ensure(t.bytes[m] + 32));
 		const void* from = src[m];
-		if(!pinned(from)) { CK(t.h_text[m].ensure(t.bytes[m])); memcpy(t.h_text[m].p, from, t.bytes[m]); from = t.h_text[m].p; }
+		if(!is_pinned(from)) { CK(t.h_text[m].ensure(t.bytes[m])); memcpy(t.h_text[m].p, from, t.bytes[m]); from = t.h_text[m].p; }
 		CK(cudaMemcpyAsync(t.d_text[m].p, from, t.bytes[m], cudaMemcpyHostToDevice, s.st));
 		const uint32_t tiles = (uint32_t)((t.bytes[m] + kTextTile - 1) / kTextTile);
 		CK(t.tile_cnt[m].ensure(tiles)); CK(t.tile_off[m].ensure(tiles + 1)); CK(t.nl[m].ensure(n * L + 1));

@@ -3,10 +3,12 @@
 #include "../../include/cfb200.h"
 #include "cf_index.h"
 #include "cf_kernels.cuh"
+#include "cf_buf.cuh"
 #include <cub/cub.cuh>
 
 #include <algorithm>
 #include <atomic>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <fcntl.h>
@@ -1187,49 +1189,30 @@ extern "C" const char* cfb_last_error(void) { return g_err; }
 int cfb_fail_msg(int code, const char* msg) { return fail(code, "%s", msg); }      // for the other translation units (cf_gunzip.cu)
 extern "C" const char* cfb_version(void) { return "cfb200 0.1 (sm_90a)"; }
 
-template <class T> struct DBuf {     // growable device buffer
-	T* p = nullptr; size_t cap = 0;
-	cudaError_t ensure(size_t n) {
-		if(n <= cap) return cudaSuccess;
-		if(p) cudaFree(p);
-		p = nullptr; cap = 0;
-		size_t want = n + n / 8 + 16;
-		cudaError_t e = cudaMalloc((void**)&p, want * sizeof(T));
-		if(e == cudaSuccess) cap = want;
-		return e;
-	}
-	void release() { if(p) cudaFree(p); p = nullptr; cap = 0; }
-};
-template <class T> struct HBuf {     // growable pinned host buffer
-	T* p = nullptr; size_t cap = 0;
-	cudaError_t ensure(size_t n) {
-		if(n <= cap) return cudaSuccess;
-		if(p) cudaFreeHost(p);
-		p = nullptr; cap = 0;
-		size_t want = n + n / 8 + 16;
-		cudaError_t e = cudaMallocHost((void**)&p, want * sizeof(T));
-		if(e == cudaSuccess) cap = want;
-		return e;
-	}
-	void release() { if(p) cudaFreeHost(p); p = nullptr; cap = 0; }
-};
-
 struct cfb_index {
 	HostIndex h;
 	int device = -1;
 	IndexView view;            // device pointers (taxonomy-independent part)
-	std::vector<void*> dptrs;
+	std::vector<DBuf<uint8_t>> dptrs;
 	uint64_t device_bytes = 0;
 	int sm_count = 0;
 	cfb_index_tables tables;
 	cfb_index() { memset(&tables, 0, sizeof tables); }
+	~cfb_index() { if(!dptrs.empty()) cudaSetDevice(device); }
+	// a device array of the replica: `bytes` allocated, `counted` of them reported in device_bytes
+	template <class T> cudaError_t alloc(size_t bytes, uint64_t counted, T** out) {
+		DBuf<uint8_t> b;
+		const cudaError_t e = b.alloc(bytes);
+		if(e != cudaSuccess) return e;
+		*out = (T*)b.p; dptrs.push_back(std::move(b)); device_bytes += counted;
+		return cudaSuccess;
+	}
 };
 
 static int upload(cfb_index* ix, const void* src, size_t bytes, const void** dst) {
 	void* d = nullptr;
-	CK(cudaMalloc(&d, bytes ? bytes : 16));
+	CK(ix->alloc(bytes ? bytes : 16, bytes, &d));
 	if(bytes) CK(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
-	ix->dptrs.push_back(d); ix->device_bytes += bytes;
 	*dst = d;
 	return CFB_OK;
 }
@@ -1238,16 +1221,16 @@ static int upload(cfb_index* ix, const void* src, size_t bytes, const void** dst
 // the previous one is on its way over PCIe.  No host copy of the array is kept.
 static int stream_to_device(cfb_index* ix, const std::string& path, uint64_t off, uint64_t bytes, const void** dst) {
 	void* d = nullptr;
-	CK(cudaMalloc(&d, bytes ? bytes + 64 : 64));
-	ix->dptrs.push_back(d); ix->device_bytes += bytes; *dst = d;
+	CK(ix->alloc(bytes + 64, bytes, &d));
+	*dst = d;
 	if(bytes == 0) return CFB_OK;
 	const int fd = open(path.c_str(), O_RDONLY);
 	if(fd < 0) return fail(CFB_EIO, "could not open %s", path.c_str());
 	const size_t kBuf = 64u << 20; const int kRing = 3, kThreads = 8;
-	uint8_t* hb[kRing] = {nullptr, nullptr, nullptr}; cudaEvent_t ev[kRing]; cudaStream_t st = nullptr;
+	HBuf<uint8_t> hb[kRing]; Event ev[kRing]; Stream st;
 	int rc = CFB_OK;
-	for(int i = 0; i < kRing; i++) { if(cudaMallocHost((void**)&hb[i], kBuf) != cudaSuccess || cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess) rc = fail(CFB_ENOMEM, "pinned staging buffers"); }
-	if(rc == CFB_OK && cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) rc = fail(CFB_ECUDA, "stream");
+	for(int i = 0; i < kRing; i++) { if(hb[i].alloc(kBuf) != cudaSuccess || ev[i].create(cudaEventDisableTiming) != cudaSuccess) rc = fail(CFB_ENOMEM, "pinned staging buffers"); }
+	if(rc == CFB_OK && st.create() != cudaSuccess) rc = fail(CFB_ECUDA, "stream");
 	uint64_t done = 0; int k = 0;
 	while(rc == CFB_OK && done < bytes) {
 		const size_t n = (size_t)std::min<uint64_t>(kBuf, bytes - done);
@@ -1256,38 +1239,35 @@ static int stream_to_device(cfb_index* ix, const std::string& path, uint64_t off
 		std::atomic<bool> bad(false);
 		auto piece = [&](int t) {
 			const size_t lo = n * t / kThreads, hi = n * (t + 1) / kThreads; size_t got = lo;
-			while(got < hi) { const ssize_t r = pread(fd, hb[b] + got, hi - got, (off_t)(off + done + got)); if(r <= 0) { bad = true; return; } got += (size_t)r; }
+			while(got < hi) { const ssize_t r = pread(fd, hb[b].p + got, hi - got, (off_t)(off + done + got)); if(r <= 0) { bad = true; return; } got += (size_t)r; }
 		};
 		std::vector<std::thread> th;
 		for(int t = 1; t < kThreads; t++) th.emplace_back(piece, t);
 		piece(0);
 		for(size_t t = 0; t < th.size(); t++) th[t].join();
 		if(bad) { rc = fail(CFB_EIO, "short read in %s", path.c_str()); break; }
-		if(cudaMemcpyAsync((uint8_t*)d + done, hb[b], n, cudaMemcpyHostToDevice, st) != cudaSuccess || cudaEventRecord(ev[b], st) != cudaSuccess) { rc = fail(CFB_ECUDA, "H2D of %s", path.c_str()); break; }
+		if(cudaMemcpyAsync((uint8_t*)d + done, hb[b].p, n, cudaMemcpyHostToDevice, st) != cudaSuccess || cudaEventRecord(ev[b], st) != cudaSuccess) { rc = fail(CFB_ECUDA, "H2D of %s", path.c_str()); break; }
 		done += n; k++;
 	}
-	if(st) { if(cudaStreamSynchronize(st) != cudaSuccess && rc == CFB_OK) rc = fail(CFB_ECUDA, "H2D of %s", path.c_str()); cudaStreamDestroy(st); }
-	for(int i = 0; i < kRing; i++) { if(hb[i]) cudaFreeHost(hb[i]); cudaEventDestroy(ev[i]); }
+	if(st && cudaStreamSynchronize(st) != cudaSuccess && rc == CFB_OK) rc = fail(CFB_ECUDA, "H2D of %s", path.c_str());
 	close(fd);
 	return rc;
 }
 
-// CK inside the loader: the half-built replica is released before the error is returned
-#define CKX(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { const int rc_ = fail(CFB_ECUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); cfb_index_free(ix); return rc_; } } while(0)
 extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flags, cfb_index** out) {
 	if(!basename || !out) return fail(CFB_EINVAL, "cfb_index_load: null argument");
-	cfb_index* ix = new cfb_index();
+	std::unique_ptr<cfb_index> ix(new cfb_index());       // the half-built replica goes with every error return
 	std::string err = load_cf_index(basename, ix->h, /*defer_bulk=*/device >= 0);
-	if(!err.empty()) { delete ix; return fail(CFB_EIO, "%s", err.c_str()); }
+	if(!err.empty()) return fail(CFB_EIO, "%s", err.c_str());
 	const HostIndex& h = ix->h;
 	ix->device = device;
 	if(device >= 0) {
-		if(h.line_rate != 7) { const int lr = h.line_rate; delete ix; return fail(CFB_EFORMAT, "index lineRate %d unsupported: the kernels require 128-byte sides (centrifuge-build default --linerate 7)", lr); }
-		if(h.ftab_chars > 15) { const int fc = h.ftab_chars; delete ix; return fail(CFB_EFORMAT, "ftabChars %d unsupported", fc); }
+		if(h.line_rate != 7) return fail(CFB_EFORMAT, "index lineRate %d unsupported: the kernels require 128-byte sides (centrifuge-build default --linerate 7)", h.line_rate);
+		if(h.ftab_chars > 15) return fail(CFB_EFORMAT, "ftabChars %d unsupported", h.ftab_chars);
 		int ndev = 0;
-		if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= device) { delete ix; return fail(CFB_ENODEV, "no CUDA device %d (found %d); this library has no CPU fallback", device, ndev); }
+		if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= device) return fail(CFB_ENODEV, "no CUDA device %d (found %d); this library has no CPU fallback", device, ndev);
 		cudaDeviceProp prop;
-		if(cudaSetDevice(device) != cudaSuccess || cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ix; return fail(CFB_ENODEV, "cannot use CUDA device %d", device); }
+		if(cudaSetDevice(device) != cudaSuccess || cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(CFB_ENODEV, "cannot use CUDA device %d", device);
 		ix->sm_count = prop.multiProcessorCount;
 		IndexView& v = ix->view; memset(&v, 0, sizeof v);
 		int rc;
@@ -1304,19 +1284,17 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 		const int layout = choose_rank_layout(free0, h.num_sides, sample_b, fixed_b, headroom0, er && er[0] == '0');
 		if(layout == kLayoutNone) {
 			const unsigned long long nr = rank16_bytes_for(h.num_sides) + h.num_sides * 128, nc = cr_bytes_for(h.num_sides), rest = sample_b + fixed_b + headroom0;
-			delete ix;
 			return fail(CFB_ENOMEM, "index %s fits no rank layout on device %d: rank16 needs %llu bytes and the compact layout %llu, each plus %llu bytes "
 			            "of sample, fixed tables and head-room; %llu bytes are free", basename, device, nr + rest, nc + rest, rest, (unsigned long long)free0);
 		}
-		#define UP(field, vec, T) if((rc = upload(ix, (vec).data(), (vec).size() * sizeof(T), (const void**)&v.field)) != CFB_OK) { cfb_index_free(ix); return rc; }
-		if((rc = stream_to_device(ix, std::string(basename) + ".1.cf", h.sides_file_off, h.num_sides * h.side_sz, (const void**)&v.sides)) != CFB_OK) { cfb_index_free(ix); return rc; }
+		auto up = [&](const auto& vec, auto*& field) { return upload(ix.get(), vec.data(), vec.size() * sizeof(vec[0]), (const void**)&field); };
 		ix->tables.sample_bytes = h.offs_len * (h.wide_sample ? 4 : 2);
-		UP(ftab, h.ftab, uint64_t) UP(eftab, h.eftab, uint64_t)
-		if((rc = stream_to_device(ix, std::string(basename) + ".2.cf", h.sample_file_off, h.offs_len * (h.wide_sample ? 4 : 2),
-		                          h.wide_sample ? (const void**)&v.sample32 : (const void**)&v.sample16)) != CFB_OK) { cfb_index_free(ix); return rc; }
-		UP(brow, h.brow, uint64_t) UP(bseq, h.bseq, uint32_t) UP(bbits, h.bbits, uint32_t)
-		UP(seq_taxid, h.seq_taxid, uint64_t) UP(seq_path, h.seq_path, int32_t) UP(paths, h.paths, uint64_t)
-		#undef UP
+		if((rc = stream_to_device(ix.get(), std::string(basename) + ".1.cf", h.sides_file_off, h.num_sides * h.side_sz, (const void**)&v.sides)) ||
+		   (rc = up(h.ftab, v.ftab)) || (rc = up(h.eftab, v.eftab)) ||
+		   (rc = stream_to_device(ix.get(), std::string(basename) + ".2.cf", h.sample_file_off, h.offs_len * (h.wide_sample ? 4 : 2),
+		                          h.wide_sample ? (const void**)&v.sample32 : (const void**)&v.sample16)) ||
+		   (rc = up(h.brow, v.brow)) || (rc = up(h.bseq, v.bseq)) || (rc = up(h.bbits, v.bbits)) ||
+		   (rc = up(h.seq_taxid, v.seq_taxid)) || (rc = up(h.seq_path, v.seq_path)) || (rc = up(h.paths, v.paths))) return rc;
 		v.len = h.len; v.zoff = h.zoff; v.zside = h.zoff / 384; v.zoffc = (uint32_t)(h.zoff % 384);
 		for(int i = 0; i < 4; i++) v.fchr[i] = h.fchr[i];
 		v.last_boundary = h.last_boundary; v.num_sides = h.num_sides;
@@ -1328,22 +1306,19 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 			if(compact) {
 				const uint64_t nsb = cr_superblocks(h.num_sides);
 				uint64_t* sb = nullptr;
-				CKX(cudaMalloc((void**)&sb, nsb * 32));
-				ix->dptrs.push_back(sb); ix->device_bytes += nsb * 32;
+				CK(ix->alloc(nsb * 32, nsb * 32, &sb));
 				k_cr_superblocks<<<(unsigned)((nsb + 255) / 256), 256>>>(v.sides, h.num_sides, h.zoff, nsb, sb);
 				k_cr_convert<<<(unsigned)((h.num_sides + 255) / 256), 256>>>(const_cast<uint64_t*>(v.sides), h.num_sides, h.zoff, sb);
 				v.crsb = sb;
 			} else {
-				CKX(cudaMalloc((void**)&r16, (nb + 1) * 64));
-				ix->dptrs.push_back(r16); ix->device_bytes += (nb + 1) * 64;
+				CK(ix->alloc((nb + 1) * 64, (nb + 1) * 64, &r16));
 				k_build_rank16<<<(unsigned)((nb + 1 + 255) / 256), 256>>>(v.sides, h.num_sides, v.zside, v.zoffc, r16);
 				if(v.n_boundaries) k_mark_boundaries<<<(v.n_boundaries + 255) / 256, 256>>>(v.brow, v.n_boundaries, r16);
 			}
 			uint64_t* f2 = nullptr; const uint64_t nf = h.ftab_len - 1;
-			CKX(cudaMalloc((void**)&f2, nf * 16));
-			ix->dptrs.push_back(f2); ix->device_bytes += nf * 16;
+			CK(ix->alloc(nf * 16, nf * 16, &f2));
 			k_build_ftab2<<<(unsigned)((nf + 255) / 256), 256>>>(v, nf, f2);
-			CKX(cudaDeviceSynchronize());
+			CK(cudaDeviceSynchronize());
 			v.ftab2 = f2; ix->tables.ftab2_bytes = nf * 16;
 			if(compact) {      // the converted sides are the rank structure: sides_bytes reports them
 				v.cr = v.sides; v.sides = nullptr;
@@ -1353,8 +1328,7 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 				ix->tables.rank16_bytes = (nb + 1) * 64;
 				// The file's sides were only the staging buffer of rank16, which holds the same information (the scalar LF of the
 				// extension step reads rank16 too): no kernel reads them from here on.
-				cudaFree((void*)v.sides);
-				ix->dptrs.erase(std::find(ix->dptrs.begin(), ix->dptrs.end(), (void*)v.sides));
+				ix->dptrs.erase(std::find_if(ix->dptrs.begin(), ix->dptrs.end(), [&](const DBuf<uint8_t>& b) { return (const void*)b.p == (const void*)v.sides; }));
 				ix->device_bytes -= h.num_sides * h.side_sz; v.sides = nullptr;
 			}
 			// HBM budget of the derived tables: what is free now minus the head-room the batch buffers need (12 GB by default, 15 % of an
@@ -1380,10 +1354,9 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 				const uint64_t nk = K ? 1ull << (2 * K) : 0;
 				if(K && h.len + 1 < (1ull << 40) && nk * 16 <= budget()) {
 					ulonglong2* fk = nullptr;
-					CKX(cudaMalloc((void**)&fk, nk * 16));
-					ix->dptrs.push_back(fk); ix->device_bytes += nk * 16;
+					CK(ix->alloc(nk * 16, nk * 16, &fk));
 					k_build_ftabk<<<(unsigned)((nk + 127) / 128), 128>>>(v, K, nk, death, fk);
-					CKX(cudaDeviceSynchronize());
+					CK(cudaDeviceSynchronize());
 					v.ftabk = (const uint64_t*)fk; v.ftabk_chars = K; v.ftabd_chars = death ? K + 3 : 0;
 					ix->tables.ftabk_bytes = nk * 16; ix->tables.ftabk_chars = K; ix->tables.ftabd_chars = v.ftabd_chars;
 				}
@@ -1394,17 +1367,15 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 				const char* e = (flags & CFB_LOAD_NO_RESOLVE_TABLE) ? "0" : getenv("CFB_RESOLVE_TABLE");
 				const uint64_t nrows = h.len + 1, esz = h.wide_sample ? 4 : 2;
 				if(!(e && e[0] == '0') && nrows * esz + 16 <= budget()) {
-					void* tab = nullptr; unsigned long long* sc = nullptr;
-					CKX(cudaMalloc(&tab, nrows * esz + 16)); CKX(cudaMalloc((void**)&sc, 16));
-					ix->dptrs.push_back(tab); ix->device_bytes += nrows * esz;
+					void* tab = nullptr; DBuf<unsigned long long> sc;
+					CK(ix->alloc(nrows * esz + 16, nrows * esz, &tab)); CK(sc.alloc(2));
 					const unsigned long long init[2] = {0ull, (unsigned long long)nrows};
-					CKX(cudaMemcpy(sc, init, 16, cudaMemcpyHostToDevice));
+					CK(cudaMemcpy(sc.p, init, 16, cudaMemcpyHostToDevice));
 					ResolveArgs ra; ra.v = v; ra.rows = nullptr; ra.ids = h.wide_sample ? (uint32_t*)tab : nullptr; ra.ids16 = h.wide_sample ? nullptr : (uint16_t*)tab;
-					ra.total = (const uint64_t*)(sc + 1); ra.rows_cap = nrows; ra.task_ctr = sc; ra.chunk = 256; ra.ctr = nullptr;
+					ra.total = (const uint64_t*)(sc.p + 1); ra.rows_cap = nrows; ra.task_ctr = sc.p; ra.chunk = 256; ra.ctr = nullptr;
 					int occ = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_resolve_c<false, true>, kSearchThreads, 0);
 					k_resolve_c<false, true><<<prop.multiProcessorCount * std::max(occ, 1), kSearchThreads>>>(ra);
-					CKX(cudaDeviceSynchronize());
-					cudaFree(sc);
+					CK(cudaDeviceSynchronize());
 					if(h.wide_sample) v.rtab32 = (const uint32_t*)tab; else v.rtab16 = (const uint16_t*)tab;
 					ix->tables.resolve_table_bytes = nrows * esz; ix->tables.resolve_entry_bytes = (int32_t)esz;
 				}
@@ -1417,11 +1388,10 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 				{ const char* f = getenv("CFB_WALK8_ROWS"); if(f) cover = std::min<uint64_t>(nrows, strtoull(f, NULL, 10)); }     // tests: force a partial table
 				if(!(e && e[0] == '0') && nrows < (1ull << 40) && cover >= nrows / 8 && cover > 0) {
 					void* tab = nullptr;
-					CKX(cudaMalloc(&tab, cover * 8 + 16));
-					ix->dptrs.push_back(tab); ix->device_bytes += cover * 8;
+					CK(ix->alloc(cover * 8 + 16, cover * 8, &tab));
 					int occ = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_build_walk8, kSearchThreads, 0);
 					k_build_walk8<<<prop.multiProcessorCount * std::max(occ, 1) * 4, kSearchThreads>>>(v, cover, (uint64_t*)tab);
-					CKX(cudaDeviceSynchronize());
+					CK(cudaDeviceSynchronize());
 					v.walk8 = (const uint64_t*)tab; v.walk8_rows = cover;
 					ix->tables.walk8_bytes = cover * 8; ix->tables.walk8_rows = cover;
 				}
@@ -1431,16 +1401,11 @@ extern "C" int cfb_index_load_ex(const char* basename, int device, uint32_t flag
 		// host copies of the big arrays are no longer needed once uploaded
 		std::vector<uint8_t>().swap(ix->h.sides);
 	}
-	*out = ix;
+	*out = ix.release();
 	return CFB_OK;
 }
-#undef CKX
 extern "C" int cfb_index_load(const char* basename, int device, cfb_index** out) { return cfb_index_load_ex(basename, device, 0u, out); }
-extern "C" void cfb_index_free(cfb_index* ix) {
-	if(!ix) return;
-	if(ix->device >= 0) { cudaSetDevice(ix->device); for(size_t i = 0; i < ix->dptrs.size(); i++) cudaFree(ix->dptrs[i]); }
-	delete ix;
-}
+extern "C" void cfb_index_free(cfb_index* ix) { delete ix; }
 extern "C" int cfb_index_get_info(const cfb_index* ix, cfb_index_info* o) {
 	if(!ix || !o) return fail(CFB_EINVAL, "null argument");
 	const HostIndex& h = ix->h;
@@ -1478,8 +1443,7 @@ extern "C" void cfb_params_default(cfb_params* p) {
 static const int kSlots = 17;  // 16 pipelined slots (two waves of 8 sub-batches keep the copy engines busy across batch boundaries) + 1 for resident batches
 
 struct Slot {
-	cudaStream_t st = nullptr;
-	cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+	Stream st; Event ev[6];
 	// inputs
 	HBuf<uint8_t> h_bases; HBuf<uint64_t> h_off; HBuf<uint32_t> h_len; HBuf<uint8_t> h_flags;
 	DBuf<uint8_t> d_bases; DBuf<uint64_t> d_off; DBuf<uint32_t> d_len; DBuf<uint8_t> d_flags;
@@ -1504,22 +1468,10 @@ struct Slot {
 	HBuf<LongTask> h_ltask; HBuf<LongUnit> h_lunit; DBuf<LongTask> d_ltask; DBuf<LongUnit> d_lunit;
 	DBuf<HitRec> lseg, lhits; DBuf<uint32_t> lsn, lsexit, lnh, lnrows, lhl; DBuf<uint64_t> lroff; DBuf<uint8_t> flags_short; DBuf<unsigned long long> lstats;
 	uint64_t lhit_slots = 0, lsegs = 0; uint32_t lntasks = 0, lmaxlen = 0;
-	void release() {
-		h_bases.release(); h_off.release(); h_len.release(); h_flags.release(); d_bases.release(); d_off.release(); d_len.release(); d_flags.release();
-		h_words.release(); d_words.release(); d_npos.release(); d_woff.release(); d_wlen.release();
-		pk.release(); nm.release(); hits.release(); nhits.release(); regen.release(); regen_n.release(); nrows.release(); row_off.release(); bsum.release(); rows.release(); ids.release(); entries.release(); tcs.release();
-		sparse.release(); nout.release(); out_off.release(); scan_tmp.release(); dense.release(); rec_off32.release(); scal.release(); h_scal.release(); h_recs.release(); h_rec_off.release(); cnt.release();
-		h_ltask.release(); h_lunit.release(); d_ltask.release(); d_lunit.release(); lseg.release(); lhits.release(); lsn.release(); lsexit.release(); lnh.release();
-		lnrows.release(); lhl.release(); lroff.release(); flags_short.release(); lstats.release();
-		for(int i = 0; i < 6; i++) if(ev[i]) cudaEventDestroy(ev[i]);
-		if(st) cudaStreamDestroy(st);
-	}
 };
 
 struct cfb_dbatch { int slot; uint64_t n_units; };
 struct TextCtx;                       // cf_text.cuh
-static void text_release(cfb_ctx*);
-static void comm_release(cfb_ctx*);   // cf_multi.cuh
 
 // Per-taxon counters of a context, on the device (SpeciesMetrics::addSpeciesCounts, aln_sink.h:142-172): for every taxid
 // the report can mention -- tree nodes, sequence taxids, 0 and 1 -- {numReads, numUniqueReads, reads whose single
@@ -1530,7 +1482,6 @@ struct CountsCtx {
 	bool ready = false;
 	std::vector<uint64_t> h_taxid; DBuf<uint64_t> d_taxid; uint32_t n = 0;
 	DBuf<unsigned long long> total, global; bool reduced = false;
-	void release() { d_taxid.release(); total.release(); global.release(); }
 };
 
 struct cfb_ctx {
@@ -1538,19 +1489,20 @@ struct cfb_ctx {
 	IndexView view; Params prm;
 	DBuf<uint64_t> d_host; DBuf<SeqInfo> d_seqs;
 	Slot slots[kSlots];
-	Counters* d_ctr = nullptr; int count = 0;        // CFB_COUNT: 1 = reference operation counters, 2 = the product's own load requests
+	DBuf<Counters> d_ctr; int count = 0;        // CFB_COUNT: 1 = reference operation counters, 2 = the product's own load requests
 	uint64_t launches = 0;
 	int resolve_blocks = 0;
 	cfb_dbatch resident; bool resident_used = false;
 	double rec_ratio = 2.0;       // records per unit seen so far (sizes the speculative D2H)
 	uint64_t rows_cap0 = 0;       // CFB_ROWS_CAP: initial row-buffer capacity (tests force the grow-and-re-run path with it)
-	TextCtx* text = nullptr;
+	std::unique_ptr<TextCtx> text;
 	CountsCtx cnt; bool fold_records = false;
 	bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
 	uint64_t long_units = 0, long_bases = 0, long_searches = 0, long_researched = 0;    // cfb_ctx_long_stats
 	uint64_t regen_lists = 0, regen_tasks = 0;   // lists regenerated / strand lists searched so far (CFB_REGEN_STATS=1 prints them when the context goes)
 	uint64_t regen_slots0 = 0;    // CFB_REGEN_SLOTS: initial capacity of the list-regeneration buffer (tests force the grow-and-re-run path with it)
-	void* comm = nullptr; int comm_rank = 0, comm_size = 1; cudaStream_t comm_st = nullptr;      // NCCL communicator (cf_multi.cuh)
+	void* comm = nullptr; int comm_rank = 0, comm_size = 1; Stream comm_st;      // NCCL communicator (cf_multi.cuh)
+	~cfb_ctx();       // after cf_multi.cuh, where TextCtx is complete
 };
 
 // every tree node whose ancestor chain contains a listed id (Classifier ctor classifier.h:157-201)
@@ -1569,27 +1521,14 @@ static void expand_taxids(const HostIndex& h, const uint64_t* ids, uint64_t n, s
 	}
 }
 
-extern "C" void cfb_ctx_destroy(cfb_ctx* c) {
-	if(!c) return;
-	if(c->ix && c->ix->device >= 0) cudaSetDevice(c->ix->device);
-	if(getenv("CFB_REGEN_STATS") && c->regen_tasks)
-		fprintf(stderr, "[cfb] strand lists regenerated by k_prep: %llu of %llu (%.3f %%)\n", (unsigned long long)c->regen_lists,
-		        (unsigned long long)c->regen_tasks, 100.0 * (double)c->regen_lists / (double)c->regen_tasks);
-	text_release(c);
-	comm_release(c);
-	c->cnt.release();
-	for(int i = 0; i < kSlots; i++) c->slots[i].release();
-	c->d_host.release(); c->d_seqs.release();
-	if(c->d_ctr) cudaFree(c->d_ctr);
-	delete c;
-}
+extern "C" void cfb_ctx_destroy(cfb_ctx* c) { delete c; }
 
 extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx** out) {
 	if(!ix || !p || !out) return fail(CFB_EINVAL, "cfb_ctx_create: null argument");
 	if(ix->device < 0) return fail(CFB_ENODEV, "index was loaded host-only; classification needs a CUDA device (no CPU fallback)");
 	if(p->khits < 1) return fail(CFB_EINVAL, "khits must be >= 1");
 	CK(cudaSetDevice(ix->device));
-	cfb_ctx* c = new cfb_ctx();
+	std::unique_ptr<cfb_ctx> c(new cfb_ctx());        // the half-built context goes with every error return
 	c->ix = ix; c->view = ix->view;
 	const HostIndex& h = ix->h;
 	Params& q = c->prm;
@@ -1602,7 +1541,6 @@ extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx*
 	std::set<uint64_t> host, excl;
 	expand_taxids(h, p->host_taxids, p->n_host_taxids, host);
 	expand_taxids(h, p->excluded_taxids, p->n_excluded_taxids, excl);
-	#define CKC(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { cfb_ctx_destroy(c); return fail(CFB_ECUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); } } while(0)
 	// the exclude set reaches the device only through the sequence table: seq_info_of reads the flags for ids < n_seqs alone
 	std::vector<uint8_t> fl;
 	if(!excl.empty()) {
@@ -1615,33 +1553,32 @@ extern "C" int cfb_ctx_create(const cfb_index* ix, const cfb_params* p, cfb_ctx*
 		hv.seq_excluded = fl.empty() ? nullptr : fl.data();
 		std::vector<SeqInfo> tab(hv.n_seqs);
 		for(uint32_t i = 0; i < hv.n_seqs; i++) tab[i] = seq_info_of(hv, q, i);
-		CKC(c->d_seqs.ensure(tab.size() + 1)); CKC(cudaMemcpy(c->d_seqs.p, tab.data(), tab.size() * sizeof(SeqInfo), cudaMemcpyHostToDevice));
+		CK(c->d_seqs.ensure(tab.size() + 1)); CK(cudaMemcpy(c->d_seqs.p, tab.data(), tab.size() * sizeof(SeqInfo), cudaMemcpyHostToDevice));
 		c->view.seqs = c->d_seqs.p;
 	}
 	if(!host.empty()) {
 		std::vector<uint64_t> hv(host.begin(), host.end());
-		CKC(c->d_host.ensure(hv.size())); CKC(cudaMemcpy(c->d_host.p, hv.data(), hv.size() * 8, cudaMemcpyHostToDevice));
+		CK(c->d_host.ensure(hv.size())); CK(cudaMemcpy(c->d_host.p, hv.data(), hv.size() * 8, cudaMemcpyHostToDevice));
 		c->view.host_taxids = c->d_host.p; c->view.n_host = (uint32_t)hv.size();
 	}
 	for(int i = 0; i < kSlots; i++) {
-		CKC(cudaStreamCreateWithFlags(&c->slots[i].st, cudaStreamNonBlocking));
-		for(int e = 0; e < 6; e++) CKC(cudaEventCreate(&c->slots[i].ev[e]));
-		CKC(c->slots[i].scal.ensure(8)); CKC(c->slots[i].h_scal.ensure(8));
+		CK(c->slots[i].st.create());
+		for(int e = 0; e < 6; e++) CK(c->slots[i].ev[e].create());
+		CK(c->slots[i].scal.ensure(8)); CK(c->slots[i].h_scal.ensure(8));
 	}
-	CKC(cudaMalloc((void**)&c->d_ctr, sizeof(Counters))); CKC(cudaMemset(c->d_ctr, 0, sizeof(Counters)));
+	CK(c->d_ctr.alloc(1)); CK(cudaMemset(c->d_ctr.p, 0, sizeof(Counters)));
 	// random 32-byte sector gathers: do not let L2 over-fetch neighbouring sectors from HBM
 	cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
 	cudaGetLastError();
 	int occ = 0;
-	CKC(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_resolve_c<false, false>, kSearchThreads, 0));
+	CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_resolve_c<false, false>, kSearchThreads, 0));
 	c->resolve_blocks = ix->sm_count * std::max(occ, 1);
 	{ const char* rc0 = getenv("CFB_ROWS_CAP"); if(rc0) c->rows_cap0 = strtoull(rc0, NULL, 10); }
 	{ const char* ks = getenv("CFB_KEEP_SHORT"); c->keep_short = ks && ks[0] == '1'; }
 	{ const char* rs = getenv("CFB_REGEN_SLOTS"); if(rs) c->regen_slots0 = strtoull(rs, NULL, 10); }
 	const char* cnt = getenv("CFB_COUNT");
 	c->count = cnt ? (cnt[0] == '1' ? 1 : (cnt[0] == '2' ? 2 : 0)) : 0;
-	#undef CKC
-	*out = c;
+	*out = c.release();
 	return CFB_OK;
 }
 extern "C" int cfb_ctx_slots(const cfb_ctx*) { return kSlots - 1; }   // last slot is reserved for resident batches
@@ -1771,23 +1708,18 @@ static int stage_batch(cfb_ctx* c, Slot& s, const cfb_batch* b) {
 	CKL(s.d_bases.ensure(b->n_bases + 16), "the bases"); CK(s.d_off.ensure(n * nm)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
 	// Caller arrays that already live in pinned memory (cfb_host_alloc) are DMA'd from where they are and
 	// must stay untouched until cfb_classify_wait; pageable arrays are staged through pinned buffers first.
-	auto pinned = [](const void* p) -> bool {
-		cudaPointerAttributes at;
-		if(cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
-		return at.type == cudaMemoryTypeHost;
-	};
 	const uint8_t* src_bases = b->bases;
-	if(!pinned(b->bases)) { CK(s.h_bases.ensure(b->n_bases)); memcpy(s.h_bases.p, b->bases, b->n_bases); src_bases = s.h_bases.p; }
+	if(!is_pinned(b->bases)) { CK(s.h_bases.ensure(b->n_bases)); memcpy(s.h_bases.p, b->bases, b->n_bases); src_bases = s.h_bases.p; }
 	CK(cudaMemcpyAsync(s.d_bases.p, src_bases, b->n_bases, cudaMemcpyHostToDevice, s.st));
 	CK(s.h_off.ensure(n * nm)); CK(s.h_len.ensure(n * nm)); CK(s.h_flags.ensure(n));
 	for(int m = 0; m < nm; m++) {
 		const uint64_t* so = b->off[m]; const uint32_t* sl = b->len[m];
-		if(!pinned(so)) { memcpy(s.h_off.p + m * n, so, n * 8); so = s.h_off.p + m * n; }
-		if(!pinned(sl)) { memcpy(s.h_len.p + m * n, sl, n * 4); sl = s.h_len.p + m * n; }
+		if(!is_pinned(so)) { memcpy(s.h_off.p + m * n, so, n * 8); so = s.h_off.p + m * n; }
+		if(!is_pinned(sl)) { memcpy(s.h_len.p + m * n, sl, n * 4); sl = s.h_len.p + m * n; }
 		CK(cudaMemcpyAsync(s.d_off.p + m * n, so, n * 8, cudaMemcpyHostToDevice, s.st));
 		CK(cudaMemcpyAsync(s.d_len.p + m * n, sl, n * 4, cudaMemcpyHostToDevice, s.st));
 	}
-	if(b->flags && pinned(b->flags)) CK(cudaMemcpyAsync(s.d_flags.p, b->flags, n, cudaMemcpyHostToDevice, s.st));
+	if(b->flags && is_pinned(b->flags)) CK(cudaMemcpyAsync(s.d_flags.p, b->flags, n, cudaMemcpyHostToDevice, s.st));
 	else { if(b->flags) memcpy(s.h_flags.p, b->flags, n); else memset(s.h_flags.p, 3, n); CK(cudaMemcpyAsync(s.d_flags.p, s.h_flags.p, n, cudaMemcpyHostToDevice, s.st)); }
 	s.bv.bases = s.d_bases.p; s.bv.flags = s.d_flags.p; s.bv.n_units = (uint32_t)n; s.bv.n_mates = nm;
 	for(int m = 0; m < 2; m++) { s.bv.off[m] = m < nm ? s.d_off.p + m * n : nullptr; s.bv.len[m] = m < nm ? s.d_len.p + m * n : nullptr; }
@@ -1849,26 +1781,21 @@ static int stage_batch_packed(cfb_ctx* c, Slot& s, const cfb_batch_packed* b) {
 	const uint64_t scan_blocks = (n + kScanBlock * kScanPer - 1) / (kScanBlock * kScanPer);
 	CKL(s.d_bases.ensure(b->n_words * 32 + 64), "the bases"); CK(s.d_off.ensure(n * nm + 1)); CK(s.d_len.ensure(n * nm)); CK(s.d_flags.ensure(n));
 	CKL(s.d_words.ensure(b->n_words + 1), "the packed bases"); CK(s.d_npos.ensure(b->n_n + 1)); CK(s.d_wlen.ensure(n + 1)); CK(s.d_woff.ensure(n + 2)); CK(s.bsum.ensure(scan_blocks + 1));
-	auto pinned = [](const void* p) -> bool {
-		cudaPointerAttributes at;
-		if(cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return false; }
-		return at.type == cudaMemoryTypeHost;
-	};
 	const uint64_t* src_words = b->words;
-	if(!pinned(b->words)) { CK(s.h_words.ensure(b->n_words)); memcpy(s.h_words.p, b->words, b->n_words * 8); src_words = s.h_words.p; }
+	if(!is_pinned(b->words)) { CK(s.h_words.ensure(b->n_words)); memcpy(s.h_words.p, b->words, b->n_words * 8); src_words = s.h_words.p; }
 	CK(cudaMemcpyAsync(s.d_words.p, src_words, b->n_words * 8, cudaMemcpyHostToDevice, s.st));
 	CK(s.h_len.ensure(n * nm)); CK(s.h_flags.ensure(n));
 	for(int m = 0; m < nm; m++) {
 		const uint32_t* sl = b->len[m];
-		if(!pinned(sl)) { memcpy(s.h_len.p + m * n, sl, n * 4); sl = s.h_len.p + m * n; }
+		if(!is_pinned(sl)) { memcpy(s.h_len.p + m * n, sl, n * 4); sl = s.h_len.p + m * n; }
 		CK(cudaMemcpyAsync(s.d_len.p + m * n, sl, n * 4, cudaMemcpyHostToDevice, s.st));
 	}
 	if(b->n_n) {
 		const uint64_t* sp = b->n_pos;
-		if(!pinned(sp)) { CK(s.h_off.ensure(b->n_n)); memcpy(s.h_off.p, sp, b->n_n * 8); sp = s.h_off.p; }
+		if(!is_pinned(sp)) { CK(s.h_off.ensure(b->n_n)); memcpy(s.h_off.p, sp, b->n_n * 8); sp = s.h_off.p; }
 		CK(cudaMemcpyAsync(s.d_npos.p, sp, b->n_n * 8, cudaMemcpyHostToDevice, s.st));
 	}
-	if(b->flags && pinned(b->flags)) CK(cudaMemcpyAsync(s.d_flags.p, b->flags, n, cudaMemcpyHostToDevice, s.st));
+	if(b->flags && is_pinned(b->flags)) CK(cudaMemcpyAsync(s.d_flags.p, b->flags, n, cudaMemcpyHostToDevice, s.st));
 	else { if(b->flags) memcpy(s.h_flags.p, b->flags, n); else memset(s.h_flags.p, 3, n); CK(cudaMemcpyAsync(s.d_flags.p, s.h_flags.p, n, cudaMemcpyHostToDevice, s.st)); }
 	// expand on the device
 	const uint32_t W = (maxlen + 31) / 32;
@@ -1980,11 +1907,11 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	s.dense_cap = s.rows_cap; CK(s.dense.ensure(s.dense_cap));
 	CK(cudaMemsetAsync(s.scal.p, 0, 4 * sizeof(unsigned long long), s.st));   // task counters, overflow flag, row allocator; [4] is rewritten by the scan
 	if(time_it) CK(cudaEventRecord(s.ev[0], s.st));
-	Counters* ctr = c->count ? c->d_ctr : nullptr;
-	if(c->count && stage == 0) CK(cudaMemsetAsync(c->d_ctr, 0, sizeof(Counters), s.st));
+	Counters* ctr = c->count ? c->d_ctr.p : nullptr;
+	if(c->count && stage == 0) CK(cudaMemsetAsync(c->d_ctr.p, 0, sizeof(Counters), s.st));
 	else if(c->count) {      // a re-run from the row stage scores every unit again: its k_score statistics start over
 		const size_t sc0 = offsetof(Counters, sc_units);
-		CK(cudaMemsetAsync(reinterpret_cast<char*>(c->d_ctr) + sc0, 0, sizeof(Counters) - sc0, s.st));
+		CK(cudaMemsetAsync(reinterpret_cast<char*>(c->d_ctr.p) + sc0, 0, sizeof(Counters) - sc0, s.st));
 	}
 	UnitArgs ua; ua.v = c->view; ua.p = c->prm; ua.b = sb; ua.hits = s.hits.p; ua.nhits = s.nhits.p; ua.cap = s.cap;
 	ua.nrows = s.nrows.p; ua.row_off = s.row_off.p; ua.row_total = s.scal.p + 3; ua.rows = s.rows.p; ua.ids = s.ids.p; ua.rows_cap = s.rows_cap;
@@ -2239,7 +2166,7 @@ extern "C" int cfb_ctx_long_stats(const cfb_ctx* c, uint64_t out[4]) {
 extern "C" int cfb_ctx_counters(cfb_ctx* c, uint64_t out[8]) {
 	if(!c || !out) return fail(CFB_EINVAL, "null argument");
 	CK(cudaSetDevice(c->ix->device));
-	Counters h; CK(cudaMemcpy(&h, c->d_ctr, sizeof h, cudaMemcpyDeviceToHost));
+	Counters h; CK(cudaMemcpy(&h, c->d_ctr.p, sizeof h, cudaMemcpyDeviceToHost));
 	out[0] = h.units; out[1] = h.partial_searches; out[2] = h.ftab_probes; out[3] = h.sides_search;
 	out[4] = h.walk_steps; out[5] = h.rows_resolved; out[6] = h.lf_steps; out[7] = h.ext_searches;
 	return CFB_OK;
@@ -2253,31 +2180,39 @@ extern "C" void cfb_host_free(void* p) { if(p) cudaFreeHost(p); }
 extern "C" int cfb_test_lf(const cfb_index* ix, const uint64_t* rows, const uint8_t* chars, uint64_t n, uint64_t* out) {
 	if(!ix || ix->device < 0) return fail(CFB_ENODEV, "no device");
 	CK(cudaSetDevice(ix->device));
-	uint64_t *dr = nullptr, *dout = nullptr; uint8_t* dc = nullptr;
-	CK(cudaMalloc(&dr, n * 8 + 8)); CK(cudaMalloc(&dout, n * 8 + 8)); CK(cudaMalloc(&dc, n + 8));
-	CK(cudaMemcpy(dr, rows, n * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dc, chars, n, cudaMemcpyHostToDevice));
-	k_test_lf<<<64, 128>>>(ix->view, dr, dc, n, dout);
+	DBuf<uint64_t> dr, dout; DBuf<uint8_t> dc;
+	CK(dr.alloc(n + 1)); CK(dout.alloc(n + 1)); CK(dc.alloc(n + 8));
+	CK(cudaMemcpy(dr.p, rows, n * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dc.p, chars, n, cudaMemcpyHostToDevice));
+	k_test_lf<<<64, 128>>>(ix->view, dr.p, dc.p, n, dout.p);
 	CK(cudaDeviceSynchronize());
-	CK(cudaMemcpy(out, dout, n * 8, cudaMemcpyDeviceToHost));
-	cudaFree(dr); cudaFree(dout); cudaFree(dc);
+	CK(cudaMemcpy(out, dout.p, n * 8, cudaMemcpyDeviceToHost));
 	return CFB_OK;
 }
 extern "C" int cfb_test_resolve(const cfb_index* ix, const uint64_t* rows, uint64_t n, uint32_t* out) {
 	if(!ix || ix->device < 0) return fail(CFB_ENODEV, "no device");
 	CK(cudaSetDevice(ix->device));
-	uint64_t* dr = nullptr; uint32_t* dout = nullptr; unsigned long long* sc = nullptr;
-	CK(cudaMalloc(&dr, n * 8 + 8)); CK(cudaMalloc(&dout, n * 4 + 8)); CK(cudaMalloc(&sc, 16));
-	CK(cudaMemcpy(dr, rows, n * 8, cudaMemcpyHostToDevice));
+	DBuf<uint64_t> dr; DBuf<uint32_t> dout; DBuf<unsigned long long> sc;
+	CK(dr.alloc(n + 1)); CK(dout.alloc(n + 2)); CK(sc.alloc(2));
+	CK(cudaMemcpy(dr.p, rows, n * 8, cudaMemcpyHostToDevice));
 	unsigned long long init[2] = {0ull, (unsigned long long)n};
-	CK(cudaMemcpy(sc, init, 16, cudaMemcpyHostToDevice));
-	ResolveArgs ra; ra.v = ix->view; ra.rows = dr; ra.ids = dout; ra.ids16 = nullptr; ra.total = (const uint64_t*)(sc + 1); ra.rows_cap = n; ra.task_ctr = sc; ra.chunk = 64; ra.ctr = nullptr;
+	CK(cudaMemcpy(sc.p, init, 16, cudaMemcpyHostToDevice));
+	ResolveArgs ra; ra.v = ix->view; ra.rows = dr.p; ra.ids = dout.p; ra.ids16 = nullptr; ra.total = (const uint64_t*)(sc.p + 1); ra.rows_cap = n; ra.task_ctr = sc.p; ra.chunk = 64; ra.ctr = nullptr;
 	if(ix->view.cr) k_resolve_c<false, false, true><<<32, kSearchThreads>>>(ra);
 	else k_resolve_c<false, false><<<32, kSearchThreads>>>(ra);
 	CK(cudaDeviceSynchronize());
-	CK(cudaMemcpy(out, dout, n * 4, cudaMemcpyDeviceToHost));
-	cudaFree(dr); cudaFree(dout); cudaFree(sc);
+	CK(cudaMemcpy(out, dout.p, n * 4, cudaMemcpyDeviceToHost));
 	return CFB_OK;
 }
 
 #include "cf_text.cuh"
 #include "cf_multi.cuh"
+
+cfb_ctx::~cfb_ctx() {
+	if(ix && ix->device >= 0) cudaSetDevice(ix->device);
+	for(int i = 0; i < kSlots; i++) if(slots[i].st) cudaStreamSynchronize(slots[i].st);
+	if(comm_st) cudaStreamSynchronize(comm_st);
+	if(getenv("CFB_REGEN_STATS") && regen_tasks)
+		fprintf(stderr, "[cfb] strand lists regenerated by k_prep: %llu of %llu (%.3f %%)\n", (unsigned long long)regen_lists,
+		        (unsigned long long)regen_tasks, 100.0 * (double)regen_lists / (double)regen_tasks);
+	if(comm && g_nccl.lib) g_nccl.CommDestroy((ncclComm_t)comm);
+}
