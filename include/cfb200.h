@@ -242,7 +242,10 @@ int cfb_text_species(cfb_ctx*, uint64_t* taxid, uint64_t* n_reads, uint64_t* n_u
  * score} for every taxid a report can mention (tree nodes, sequence taxids, 0 = unclassified, 1); the index space is
  * cfb_counts_taxids (ascending).  The text operator always counts; the record-level entry points count when
  * cfb_ctx_count_records is on (a kernel behind the classification kernels of each batch; batches add to the totals when
- * they are waited for).  cfb_counts_allreduce is the path's one collective: ncclAllReduce(ncclUint64, ncclSum) of the
+ * they are waited for).  A unit counts its records of the best score, at most -k of them.  When more than -k records tie
+ * for the best score (only under --host-taxids), the text operator picks -k of them with the read's RNG, as the
+ * reference does; the record-level counters take the first -k in record (hit-map) order, since cfb_batch carries no
+ * per-read seeds.  cfb_counts_allreduce is the path's one collective: ncclAllReduce(ncclUint64, ncclSum) of the
  * totals over the communicator, NVLink/NVSwitch underneath.  The sparse tie sets that feed the EM (cfb_text_result.multi)
  * are merged by the caller, as the reference merges `observed`. */
 int cfb_ctx_count_records(cfb_ctx*, int on);
