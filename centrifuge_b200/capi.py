@@ -5,6 +5,7 @@ fallback -- loading the library or creating a context without a usable sm_90 (H1
 """
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 
@@ -261,6 +262,10 @@ class Context:
         """Columns of the rows of later text_submit calls: a --tab-fmt-cols list ("readID,taxID,readSeq,..."); None = the
         default list.  An unknown name raises CfbError with the reference's message."""
         _ck(lib().cfb_ctx_set_columns(self.h, cols.encode() if cols is not None else None))
+
+    def set_n_ceil(self, type_, constant, coeff, min_=0.0, max_=sys.float_info.max):
+        """N ceiling of later text_submit calls (--n-ceil): type_ 1 = constant, 2 = linear, 3 = sqrt, 4 = log."""
+        _ck(lib().cfb_ctx_set_n_ceil(self.h, C.c_int(type_), C.c_double(constant), C.c_double(coeff), C.c_double(min_), C.c_double(max_)))
 
     def text_submit(self, slot, text_a, text_b=None, n_records=0, fasta=False, trim5=0, trim3=0, seed=0, maxlen_hint=0):
         """text_a/text_b: uint8 arrays of complete records (pinned arrays are DMA'd in place)."""

@@ -29,6 +29,7 @@
 // the same one the host formatter uses.
 
 #include "cf_cols.h"
+#include "cf_nceil.h"
 
 enum { TX_IRREGULAR = 1, TX_LINECOUNT = 2, TX_FMT_OVERFLOW = 4 };
 static const int kFmtMax = 32;          // records per unit the on-device selector holds
@@ -43,6 +44,7 @@ struct TextArgs {
 	uint32_t* name_off; uint32_t* id_len; uint32_t* name_len; uint32_t* seq_off[2]; uint32_t* qual_off[2];
 	uint8_t* bases;
 	unsigned long long* tscal;      // [0] status bits, [1] max length, [2] n_multi, [3] max length of the mates up to kLongUnitLen bases
+	int32_t nc_type; double nc_c, nc_l, nc_mn, nc_mx;      // N ceiling (cf_nceil.h)
 };
 
 // 16-bit mask of bytes equal to `c` in a 16-byte vector
@@ -221,7 +223,7 @@ __global__ void __launch_bounds__(128, 16) k_tok_bases(const TextArgs a) {      
 		sx = warp_xor(sx); ns = warp_add(ns);
 		const uint32_t rseed = ((a.seed + 101u) * 59u * 61u * 67u * 71u * 73u * 79u * 83u) ^ sx;
 		bool pass = len >= 2;
-		if(pass) { const uint32_t maxns = (uint32_t)(0.15 * (double)len); pass = ns <= maxns; }
+		if(pass) { bool sure; pass = nceil_pass(a.nc_type, a.nc_c, a.nc_l, a.nc_mn, a.nc_mx, len, ns, &sure); if(!sure) bad = true; }   // a log ceiling the device cannot settle: the span goes to the host reader
 		if(pass) flags |= 1u << m;
 		if(lane == 0) a.seedv[m][u] = (m == 1 && len == 0) ? 0u : rseed;
 		if(m == 0) {   // read id: drop a trailing /1 /2 /3, cut at the first whitespace (aln_sink.h:2202-2217)
@@ -469,6 +471,7 @@ struct TextSlot {
 	DBuf<unsigned long long> sp;
 	DBuf<unsigned long long> tscal; HBuf<unsigned long long> h_tscal;    // [0] status [1] maxlen [2] n_multi [3] maxlen of mates up to kLongUnitLen [4],[5] line totals [6] tsv bytes
 	uint64_t n_rec = 0; int n_mates = 1; cfb_text_opts opt; uint64_t bytes[2] = {0, 0}; bool pending = false;
+	NCeil nceil;                    // the context's N ceiling when the span was submitted (re-runs of the span keep it)
 	uint64_t spec_tsv = 0, spec_multi = 0;      // bytes / tie-set records already copied home behind the kernels
 	DBuf<uint8_t> d_cols; std::vector<uint8_t> cols;      // column list of the span in flight (device copy of `cols`)
 };
@@ -539,6 +542,13 @@ extern "C" int cfb_ctx_set_columns(cfb_ctx* c, const char* cols) {
 	return CFB_OK;
 }
 
+extern "C" int cfb_ctx_set_n_ceil(cfb_ctx* c, int type, double constant, double coeff, double min, double max) {
+	if(!c || type < NCEIL_CONST || type > NCEIL_LOG || constant != constant || coeff != coeff || min != min || max != max)
+		return fail(CFB_EINVAL, "cfb_ctx_set_n_ceil: bad argument");
+	NCeil& f = c->nceil; f.type = type; f.c = constant; f.l = coeff; f.mn = min; f.mx = max;
+	return CFB_OK;
+}
+
 static uint32_t len_class(uint32_t maxlen) { return maxlen <= 128 ? 128u : (maxlen <= 160 ? 160u : (maxlen <= 320 ? 320u : ((maxlen + 1023u) / 1024u) * 1024u)); }
 
 static int text_enqueue_format(cfb_ctx* c, Slot& s, TextSlot& t) {
@@ -602,6 +612,8 @@ static int text_enqueue_all(cfb_ctx* c, Slot& s, TextSlot& t) {
 	ta.n_rec = (uint32_t)n; ta.lines_per = L; ta.n_mates = nm; ta.fasta = t.opt.fasta ? 1 : 0; ta.trim5 = t.opt.trim5; ta.trim3 = t.opt.trim3; ta.seed = t.opt.seed;
 	ta.flags = s.d_flags.p; ta.name_off = t.name_off.p; ta.name_len = t.name_len.p; ta.id_len = t.id_len.p; ta.bases = s.d_bases.p; ta.tscal = t.tscal.p;
 	ta.maxlen_hint = s.maxlen; ta.keep_long = s.longs.empty() ? 0u : 1u;
+	ta.nc_type = t.nceil.type; ta.nc_c = t.nceil.c; ta.nc_l = t.nceil.l; ta.nc_mn = t.nceil.mn; ta.nc_mx = t.nceil.mx;
+	s.nceil = t.nceil; s.custom_nceil = !t.nceil.is_default();      // sizes the hit lists for the Ns a passing mate may hold
 	k_tok_rec<<<(unsigned)((n * nm + 127) / 128), 128, 0, s.st>>>(ta); c->launches++;
 	for(int m = 0; m < nm; m++) {
 		k_scan_sums<<<(unsigned)scan_blocks, kScanBlock, 0, s.st>>>(s.d_len.p + m * n, n, s.bsum.p);
@@ -613,7 +625,6 @@ static int text_enqueue_all(cfb_ctx* c, Slot& s, TextSlot& t) {
 	CK(cudaGetLastError());
 	s.cap = 0; s.reran = false;
 	int rc = enqueue_kernels(c, s, 0, false); if(rc) return rc;
-	(void)tc;
 	return text_enqueue_format(c, s, t);
 }
 
@@ -636,7 +647,7 @@ extern "C" int cfb_text_submit(cfb_ctx* c, int slot, const void* text_a, uint64_
 		t.cols = tc.cols;
 	}
 	const int nm = text_b ? 2 : 1; const int L = o->fasta ? 2 : 4;
-	t.n_rec = n_rec; t.n_mates = nm; t.opt = *o; t.bytes[0] = bytes_a; t.bytes[1] = text_b ? bytes_b : 0;
+	t.n_rec = n_rec; t.n_mates = nm; t.opt = *o; t.nceil = c->nceil; t.bytes[0] = bytes_a; t.bytes[1] = text_b ? bytes_b : 0;
 	s.n_units = n_rec; s.bv.n_units = (uint32_t)n_rec; s.bv.n_mates = nm; s.longs.clear(); s.win_first = 0;
 	if(n_rec == 0) { s.pending = true; t.pending = true; return CFB_OK; }
 	CK(t.tscal.ensure(8)); CK(t.h_tscal.ensure(8));

@@ -4,6 +4,7 @@
 #include "cf_index.h"
 #include "cf_kernels.cuh"
 #include "cf_buf.cuh"
+#include "cf_nceil.h"
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -1458,6 +1459,7 @@ struct Slot {
 	HBuf<OutRec> h_recs; HBuf<uint32_t> h_rec_off;
 	DBuf<unsigned long long> cnt;     // this batch's per-taxon counters (record path), added to the context's totals at wait time
 	bool folded = false, is_text = false, commit_pending = false;
+	NCeil nceil; bool custom_nceil = false;   // the batch's N ceiling when it is not the default: sizes the hit lists (nceil_full_cap)
 	// batch bookkeeping
 	BatchView bv; uint64_t n_units = 0, n_bases = 0; uint32_t maxlen = 0, cap = 0; uint64_t rows_cap = 0, dense_cap = 0;
 	bool pending = false, reran = false;
@@ -1496,6 +1498,7 @@ struct cfb_ctx {
 	double rec_ratio = 2.0;       // records per unit seen so far (sizes the speculative D2H)
 	uint64_t rows_cap0 = 0;       // CFB_ROWS_CAP: initial row-buffer capacity (tests force the grow-and-re-run path with it)
 	std::unique_ptr<TextCtx> text;
+	NCeil nceil;                  // cfb_ctx_set_n_ceil: the text operator's N filter, and the hit-list bound of every later batch
 	CountsCtx cnt; bool fold_records = false;
 	bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
 	uint64_t long_units = 0, long_bases = 0, long_searches = 0, long_researched = 0;    // cfb_ctx_long_stats
@@ -1671,6 +1674,15 @@ static int long_oom(const Slot& s, cudaError_t e, const char* what) {
 }
 // CK for buffers whose size long units drive
 #define CKL(call, what) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { if(!s.longs.empty()) return long_oom(s, e_, what); CK(e_); } } while(0)
+// Device memory for hit lists sized past the default N ceiling's bound (a custom --n-ceil, or the re-run of a batch whose
+// flags let more Ns through): CFB_ENOMEM naming the list length
+static int hits_oom(const Slot& s, cudaError_t e) {
+	cudaGetLastError();
+	return fail(CFB_ENOMEM, "no device memory for the hit lists of a batch of %llu units whose mates may hold up to %u hits per strand "
+	            "(reads up to %u bases under %s): %s", (unsigned long long)s.n_units, s.full_cap, s.maxlen,
+	            s.custom_nceil ? "a custom --n-ceil" : "filter flags that let more Ns through", cudaGetErrorString(e));
+}
+#define CKH(call) do { cudaError_t e_ = (call); if(e_ != cudaSuccess) { if(s.full_cap > s.maxlen / 4 + 8) return hits_oom(s, e_); CK(e_); } } while(0)
 
 static int mate_too_long(uint64_t n, int m, const uint32_t* L) {
 	for(uint64_t i = 0; i < n; i++)
@@ -1885,12 +1897,13 @@ static int enqueue_kernels(cfb_ctx* c, Slot& s, int stage, bool time_it) {
 	if(stage == 0) {
 		if(s.cap == 0) {
 			s.full_cap = s.maxlen / 4 + 8;      // >= #Ns allowed by the N filter (0.15 len) + len/10 + slack
+			if(s.custom_nceil) s.full_cap = nceil_full_cap(s.nceil, s.maxlen);
 			s.cap = keep_short ? s.full_cap : s.maxlen / kLongLen + 2;       // hits of >= 22 bases do not overlap
 		}
-		CK(s.hits.ensure(ntasks * s.cap)); CK(s.nhits.ensure(ntasks));
+		CKH(s.hits.ensure(ntasks * s.cap)); CK(s.nhits.ensure(ntasks));
 		if(!keep_short) {
 			s.regen_slots = std::max<uint64_t>(s.regen_slots, c->regen_slots0 ? c->regen_slots0 : std::max<uint64_t>(ntasks / 32, 1024));
-			CK(s.regen.ensure(s.regen_slots * s.full_cap)); CK(s.regen_n.ensure(s.regen_slots));
+			CKH(s.regen.ensure(s.regen_slots * s.full_cap)); CK(s.regen_n.ensure(s.regen_slots));
 			CK(cudaMemsetAsync(s.scal.p + 6, 0, sizeof(unsigned long long), s.st));
 		}
 		const uint32_t W = (s.maxlen + 31) / 32 + 1;
@@ -2017,7 +2030,7 @@ static int finish_batch(cfb_ctx* c, Slot& s, bool time_it, bool to_host, cfb_res
 			int rc = enqueue_kernels(c, s, 0, time_it); if(rc) return rc;
 			continue;
 		}
-		if(ovf == 1) {            // hit-list capacity: only possible when the caller's flags bypass the N filter
+		if(ovf == 1) {            // hit-list capacity: the caller's flags let more Ns through than the context's ceiling bounds
 			s.cap = s.maxlen + 2; s.full_cap = s.maxlen + 2; s.reran = true;
 			int rc = enqueue_kernels(c, s, 0, time_it); if(rc) return rc;
 			continue;
@@ -2065,7 +2078,7 @@ extern "C" int cfb_classify_submit(cfb_ctx* c, int slot, const cfb_batch* b) {
 	Slot& s = c->slots[slot];
 	if(s.pending) return fail(CFB_EINVAL, "slot %d still has an un-waited batch", slot);
 	int rc = stage_batch(c, s, b); if(rc) return rc;
-	s.cap = 0; s.want_host = true; s.is_text = false;
+	s.cap = 0; s.want_host = true; s.is_text = false; s.nceil = c->nceil; s.custom_nceil = !c->nceil.is_default();
 	rc = enqueue_kernels(c, s, 0, false); if(rc) return rc;
 	s.pending = true;
 	return CFB_OK;
@@ -2076,7 +2089,7 @@ extern "C" int cfb_classify_submit_packed(cfb_ctx* c, int slot, const cfb_batch_
 	Slot& s = c->slots[slot];
 	if(s.pending) return fail(CFB_EINVAL, "slot %d still has an un-waited batch", slot);
 	int rc = stage_batch_packed(c, s, b); if(rc) return rc;
-	s.cap = 0; s.want_host = true; s.is_text = false;
+	s.cap = 0; s.want_host = true; s.is_text = false; s.nceil = c->nceil; s.custom_nceil = !c->nceil.is_default();
 	rc = enqueue_kernels(c, s, 0, false); if(rc) return rc;
 	s.pending = true;
 	return CFB_OK;
@@ -2122,7 +2135,7 @@ extern "C" int cfb_batch_upload(cfb_ctx* c, const cfb_batch* b, cfb_dbatch** out
 	Slot& s = c->slots[kSlots - 1];
 	int rc = stage_batch(c, s, b); if(rc) return rc;
 	CK(cudaStreamSynchronize(s.st));
-	s.cap = 0; s.is_text = false;
+	s.cap = 0; s.is_text = false; s.nceil = c->nceil; s.custom_nceil = !c->nceil.is_default();
 	c->resident.slot = kSlots - 1; c->resident.n_units = s.n_units; c->resident_used = true;
 	*out = &c->resident;
 	return CFB_OK;
@@ -2215,4 +2228,43 @@ cfb_ctx::~cfb_ctx() {
 		fprintf(stderr, "[cfb] strand lists regenerated by k_prep: %llu of %llu (%.3f %%)\n", (unsigned long long)regen_lists,
 		        (unsigned long long)regen_tasks, 100.0 * (double)regen_lists / (double)regen_tasks);
 	if(comm && g_nccl.lib) g_nccl.CommDestroy((ncclComm_t)comm);
+}
+
+// Test hook: the device's double log and sqrt of every integer length in [lo, hi) against the host's (glibc), bit for
+// bit -- what cf_nceil.h's G and S ceilings rely on.  Counts the mismatches, and in n_log_far the logs more than one unit
+// in the last place apart; first_log: the first length whose log differs.
+__global__ void k_test_log_sqrt(uint64_t lo, uint64_t n, unsigned long long* lg, unsigned long long* sq) {
+	const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+	if(i >= n) return;
+	const double x = (double)(lo + i);
+	lg[i] = (unsigned long long)__double_as_longlong(log(x)); sq[i] = (unsigned long long)__double_as_longlong(__dsqrt_rn(x));
+}
+extern "C" int cfb_test_log_sqrt(int device, uint64_t lo, uint64_t hi, uint64_t* n_log, uint64_t* n_log_far, uint64_t* n_sqrt, uint64_t* first_log) {
+	if(!n_log || !n_log_far || !n_sqrt || !first_log || hi < lo) return fail(CFB_EINVAL, "cfb_test_log_sqrt: bad argument");
+	CK(cudaSetDevice(device));
+	const uint64_t chunk = 1ull << 26;
+	DBuf<unsigned long long> dl, ds; HBuf<unsigned long long> hl, hs;
+	CK(dl.ensure(chunk)); CK(ds.ensure(chunk)); CK(hl.ensure(chunk)); CK(hs.ensure(chunk));
+	std::atomic<uint64_t> bad_l(0), bad_s(0), far_l(0); uint64_t first = UINT64_MAX;
+	const int nth = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
+	for(uint64_t a = lo; a < hi; a += chunk) {
+		const uint64_t n = std::min(chunk, hi - a);
+		k_test_log_sqrt<<<(unsigned)((n + 255) / 256), 256>>>(a, n, dl.p, ds.p);
+		CK(cudaMemcpy(hl.p, dl.p, n * 8, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hs.p, ds.p, n * 8, cudaMemcpyDeviceToHost));
+		std::vector<uint64_t> firsts(nth, UINT64_MAX); std::vector<std::thread> th;
+		for(int t = 0; t < nth; t++) th.emplace_back([&, t]() {
+			uint64_t bl = 0, bs = 0, fl = 0;
+			for(uint64_t i = t; i < n; i += nth) {
+				const double x = (double)(a + i), l = std::log(x), s = std::sqrt(x);
+				unsigned long long ul, us; memcpy(&ul, &l, 8); memcpy(&us, &s, 8);
+				if(ul != hl.p[i]) { bl++; firsts[t] = std::min<uint64_t>(firsts[t], a + i); if(ul + 1 != hl.p[i] && ul != hl.p[i] + 1) fl++; }
+				if(us != hs.p[i]) bs++;
+			}
+			bad_l += bl; bad_s += bs; far_l += fl;
+		});
+		for(std::thread& x : th) x.join();
+		for(uint64_t f : firsts) first = std::min(first, f);
+	}
+	*n_log = bad_l; *n_log_far = far_l; *n_sqrt = bad_s; *first_log = first;
+	return CFB_OK;
 }

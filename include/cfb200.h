@@ -231,6 +231,15 @@ int cfb_text_wait(cfb_ctx*, int slot, int discard, cfb_text_result* out);
  * readID,seqID,taxID,score,2ndBestScore,hitLength,queryLength,numMatches.  Rows carry no header line.  An unknown name
  * returns CFB_EINVAL with "Column definition <name> invalid." in cfb_last_error(). */
 int cfb_ctx_set_columns(cfb_ctx*, const char* cols);
+/* N ceiling of later cfb_text_submit calls on this context (`centrifuge-class --n-ceil`): a mate of `len` bases passes
+ * the N filter when it holds at most max(min, min(max, constant + coeff * g(len))) bases N or '.', converted to an
+ * integer as the reference does, with g = 0, len, sqrt(len) or ln(len) for `type` 1 (constant), 2 (linear), 3 (square
+ * root) or 4 (natural log).  The default is type 2, constant 0, coeff 0.15, min 0, max DBL_MAX.  Mates are filtered
+ * apart.  A bad type or a NaN parameter returns CFB_EINVAL.  cfb_classify_submit callers pass their own filter flags; the
+ * ceiling still sizes the hit lists of their later batches for the Ns a passing mate may hold (a batch whose flags pass
+ * more Ns than that is re-run with lists of one entry per base).  A hit list that does not fit returns CFB_ENOMEM.
+ * A span or batch keeps the ceiling it was submitted under. */
+int cfb_ctx_set_n_ceil(cfb_ctx*, int type, double constant, double coeff, double min, double max);
 /* Per-taxon counters accumulated on the device by all accepted spans: entries with n_reads > 0.
  * n_obs1 = reads whose single best row reached the maximum score (observed keys of size 1). */
 int cfb_text_species(cfb_ctx*, uint64_t* taxid, uint64_t* n_reads, uint64_t* n_unique, uint64_t* n_obs1, uint64_t cap, uint64_t* n);
