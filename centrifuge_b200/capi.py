@@ -267,6 +267,10 @@ class Context:
         """N ceiling of later text_submit calls (--n-ceil): type_ 1 = constant, 2 = linear, 3 = sqrt, 4 = log."""
         _ck(lib().cfb_ctx_set_n_ceil(self.h, C.c_int(type_), C.c_double(constant), C.c_double(coeff), C.c_double(min_), C.c_double(max_)))
 
+    def set_quals(self, solexa=False, phred64=False, integer=False):
+        """Quality encoding of later text_submit calls (--solexa-quals, --phred64, --int-quals; all False: phred33)."""
+        _ck(lib().cfb_ctx_set_quals(self.h, C.c_int(int(solexa)), C.c_int(int(phred64)), C.c_int(int(integer))))
+
     def text_submit(self, slot, text_a, text_b=None, n_records=0, fasta=False, trim5=0, trim3=0, seed=0, maxlen_hint=0):
         """text_a/text_b: uint8 arrays of complete records (pinned arrays are DMA'd in place)."""
         o = TextOpts(1 if fasta else 0, trim5, trim3, seed, maxlen_hint)

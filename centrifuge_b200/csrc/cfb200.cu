@@ -5,6 +5,7 @@
 #include "cf_kernels.cuh"
 #include "cf_buf.cuh"
 #include "cf_nceil.h"
+#include "cf_quals.h"
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -1499,6 +1500,7 @@ struct cfb_ctx {
 	uint64_t rows_cap0 = 0;       // CFB_ROWS_CAP: initial row-buffer capacity (tests force the grow-and-re-run path with it)
 	std::unique_ptr<TextCtx> text;
 	NCeil nceil;                  // cfb_ctx_set_n_ceil: the text operator's N filter, and the hit-list bound of every later batch
+	Quals quals;                  // cfb_ctx_set_quals: the quality encoding of later text spans
 	CountsCtx cnt; bool fold_records = false;
 	bool keep_short = false;      // CFB_KEEP_SHORT=1: store every hit (A/B and tests)
 	uint64_t long_units = 0, long_bases = 0, long_searches = 0, long_researched = 0;    // cfb_ctx_long_stats

@@ -240,6 +240,12 @@ int cfb_ctx_set_columns(cfb_ctx*, const char* cols);
  * more Ns than that is re-run with lists of one entry per base).  A hit list that does not fit returns CFB_ENOMEM.
  * A span or batch keeps the ceiling it was submitted under. */
 int cfb_ctx_set_n_ceil(cfb_ctx*, int type, double constant, double coeff, double min, double max);
+/* Quality encoding of the FASTQ text of later cfb_text_submit calls (--solexa-quals, --phred64, --int-quals; all 0 is
+ * phred33, the default).  Qualities are converted to phred33 for the per-read seed and the quality columns, as the
+ * reference does (charToPhred33 / intToPhred33, qual.h:105-171); a span whose qualities the reference would refuse is
+ * returned irregular, for the record-level reader to decide.  A span keeps the encoding it was submitted under, re-runs
+ * included.  Each argument must be 0 or 1 (else CFB_EINVAL). */
+int cfb_ctx_set_quals(cfb_ctx*, int solexa, int phred64, int integer);
 /* Per-taxon counters accumulated on the device by all accepted spans: entries with n_reads > 0.
  * n_obs1 = reads whose single best row reached the maximum score (observed keys of size 1). */
 int cfb_text_species(cfb_ctx*, uint64_t* taxid, uint64_t* n_reads, uint64_t* n_unique, uint64_t* n_obs1, uint64_t cap, uint64_t* n);
